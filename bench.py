@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- batched path-QP solves/s on B200 (BASELINE.json metric), one rank per GPU.
+"""bench.py -- batched path-QP solves/s on H100 (BASELINE.json metric), one rank per GPU.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5] [--formulation KP|K|KPC]
+                  [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (QP assembly -> ADMM solve -> state extraction) over one batch of
 synthetic corridor paths.  The default workload is BASELINE config 2 (1024 paths x 100 stations per GPU);
@@ -16,13 +17,20 @@ states.  Rank 0 prints one JSON line.
                H2D + kernels + D2H inside the call, timed by host wall clock around the call
                (time.perf_counter; the library's own event spans are reported beside it as a breakdown).
   roofline     dominant kernel's algorithmic HBM bytes (SURVEY 8d: 52 N + 32 B per solve) / its average
-               launch time against the measured HBM copy bandwidth, plus the second figure SURVEY 8d
+               launch time against the HBM bandwidth measured in the same run (device-to-device copy of 256 MiB,
+               CUDA events; the H100 SXM data-sheet figure is reported beside it), plus the second figure SURVEY 8d
                mandates: the per-iteration working set W_iter = 944 N B streamed at the measured
                iteration rate, labelled ON-CHIP (the ADMM state never leaves the SM).
   cpu_baseline the CPU oracle (restatement of the reference's assembly + OSQP recurrence, oracle/) on the
                host's physical cores, bounded sample, min / median of repetitions.
   extras       default run only (config 2, one GPU): short measurements of configs 3, 4 and 5 at their
                named per-GPU sizes (QP-only, and config 3 through the chained planner iteration too).
+
+--dump-outputs DIR writes what the last timed step returned to the caller (rank 0's shard; with --impl reference the
+CPU arm's last step) as DIR/<name>.npy in float64: the output states, the Frenet states, per-path status and iteration
+count.  The inputs are a pure function of the arguments (counter-based RNG, fixed seed), so two builds can be compared
+output for output; the files total at most 64 MB (64 000 000 bytes, headers included): above that a fixed, seeded
+sample of whole paths is written (paths.npy holds their indices).
 
 --impl reference times the CPU oracle on the host cores (the reference's own OSQP-based binary cannot be
 built here: no Eigen / OSQP / osqp-eigen / glog / gflags in the image), same `config` object, same JSON
@@ -61,12 +69,9 @@ def w_iter_bytes(n):
     return 944 * n
 
 
-def measured_peak_gbs():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+HBM_DATASHEET_GBS = 3350.0   # NVIDIA H100 SXM data sheet, HBM3 (a card run below 700 W may not reach it)
+DUMP_LIMIT_BYTES = 64_000_000   # --dump-outputs: the files written, headers included, total at most this (64 MB, <= 64 MiB)
+NPY_HEADER_ALLOWANCE = 1024     # per .npy file (np.save pads its header to a multiple of 64 bytes; 128 for these arrays)
 
 
 class ClockSampler:
@@ -233,6 +238,8 @@ def run_reference(args, rank, world):
         r = cpu_solve(oracle, params, F, batch, threads)
         step_s.append(r["seconds"])
         solved += int((r["status"] == 1).sum())
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, batch["offsets"], r["states"], r["frenet"], r["status"], r["iters"])
     secs = sum(step_s)
     value = B * args.steps / secs
     line = {
@@ -466,13 +473,52 @@ def time_workload(w, torch, steps, warmup, flush, stream, barrier, with_e2e=True
     return res
 
 
-def profile_units():
-    """Measured unit utilisations of the dominant kernel from the committed ncu capture (NOT this run)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return {}
+def dump_outputs(out_dir, offsets, states, frenet, status, iters):
+    """One step's caller-visible outputs (STATE_DTYPE states, [stations, 3] Frenet states, per-path status and
+    iterations) as float64 .npy files under `out_dir`, at most DUMP_LIMIT_BYTES on disk.  When they do not fit, a fixed
+    (seeded) sample of whole paths is written instead, with their indices."""
+    os.makedirs(out_dir, exist_ok=True)
+    B = len(status)
+    n = np.diff(np.asarray(offsets, dtype=np.int64))
+    per_station = (len(STATE_DTYPE.names) + 3) * 8
+    per_path = 3 * 8                          # status, iters and (when sampled) the path index
+    budget = DUMP_LIMIT_BYTES - 5 * NPY_HEADER_ALLOWANCE
+    paths = np.arange(B)
+    if int(n.sum()) * per_station + B * per_path > budget:
+        # the longest paths first would bias the sample; draw paths uniformly and keep those that fit
+        paths = np.random.default_rng(0).permutation(B)
+        keep = np.searchsorted(np.cumsum(n[paths] * per_station + per_path), budget, side="right")
+        paths = np.sort(paths[:keep])
+    rows = np.concatenate([np.arange(offsets[i], offsets[i + 1]) for i in paths]) if len(paths) else np.zeros(0, np.int64)
+    out = {"states": np.asarray(states)[rows].view("<f8").reshape(-1, len(STATE_DTYPE.names)),
+           "frenet": np.asarray(frenet).reshape(-1, 3)[rows],
+           "status": np.asarray(status)[paths].astype(np.float64), "iters": np.asarray(iters)[paths].astype(np.float64)}
+    if len(paths) < B:
+        out["paths"] = paths.astype(np.float64)
+    files = [os.path.join(out_dir, name + ".npy") for name in out]
+    for f, arr in zip(files, out.values()):
+        np.save(f, np.ascontiguousarray(arr, dtype=np.float64))
+    written = sum(os.path.getsize(f) for f in files)
+    if written > DUMP_LIMIT_BYTES:
+        raise RuntimeError(f"--dump-outputs wrote {written} bytes, more than {DUMP_LIMIT_BYTES}")
+
+
+def measure_hbm_gbs(torch, src, reps=10):
+    """HBM bandwidth of this device, measured: a device-to-device copy of `src` (bytes read + bytes written over the
+    CUDA-event time of one copy), best of `reps`."""
+    dst = torch.empty_like(src)
+    dst.copy_(src)
+    best = None
+    for _ in range(reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        dst.copy_(src)
+        b.record()
+        b.synchronize()
+        ms = a.elapsed_time(b)
+        best = ms if best is None else min(best, ms)
+    del dst
+    return 2 * src.numel() * src.element_size() / (best * 1e-3) / 1e9
 
 
 def run_ours(args, rank, world, local_rank):
@@ -483,7 +529,7 @@ def run_ours(args, rank, world, local_rank):
     dev = torch.device("cuda", local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
     stream = torch.cuda.Stream(device=dev)  # non-default: the ABI treats a NULL stream as 'the handle's own'
     torch.cuda.set_stream(stream)
 
@@ -499,6 +545,9 @@ def run_ours(args, rank, world, local_rank):
         sampler.start()
     r = time_workload(w, torch, args.steps, args.warmup, flush, stream, barrier)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, w.batch["offsets"], np.frombuffer(w.d_out.cpu().numpy().tobytes(), dtype=STATE_DTYPE),
+                     w.d_frenet[:w.total * 3].cpu().numpy(), w.d_status.cpu().numpy(), w.d_iters.cpu().numpy())
 
     # ---- reduce over ranks: step time = max over ranks; per-rank breakdown gathered as it is
     t = torch.tensor([r["dev_ms"], r["e2e_ms"], r["wall_ms"]], dtype=torch.float64, device=dev)
@@ -533,7 +582,7 @@ def run_ours(args, rank, world, local_rank):
         steps = args.steps
         value = n_paths * steps / (dev_ms * 1e-3)
         e2e_value = n_paths * steps / (e2e_ms * 1e-3)
-        peak, peak_src = measured_peak_gbs()
+        peak = measure_hbm_gbs(torch, flush)
         mix = w.class_mix()
         dominant = max(mix, key=lambda k: mix[k])
         mean_n = w.total / w.B
@@ -542,7 +591,6 @@ def run_ours(args, rank, world, local_rank):
         achieved = alg_bytes / launch_s / 1e9
         iters_mean = float(r["iters"].mean())
         it_per_s = float(r["iters"].sum()) / launch_s
-        prof = profile_units()
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": steps,
             "warmup": args.warmup, "ms_per_step": dev_ms / steps, "higher_is_better": True,
@@ -554,18 +602,18 @@ def run_ours(args, rank, world, local_rank):
                     "kernel_launches_per_step": r["e2e_launches"]},
             "gpu_launches": r["launches_per_step"] * steps,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": prof.get("dram_bytes_per_launch") if args.config == 2 else None,
-                         "traffic_source": prof.get("source", "profiles/traffic.json") + " (ncu --set full capture of the same kernel on the same batch; not measured in this run)" if args.config == 2 else None,
-                         "peak_source": peak_src, "kernel": dominant, "kernel_classes": mix,
+                         "peak_source": "measured in this run: device-to-device copy of 256 MiB, (read + write bytes) / "
+                                        "CUDA-event time, best of 10", "datasheet_peak": HBM_DATASHEET_GBS,
+                         "datasheet_source": "NVIDIA H100 SXM data sheet, HBM3 3.35 TB/s (700 W card)",
+                         "kernel": dominant, "kernel_classes": mix,
                          "algorithmic_bytes_per_launch": alg_bytes,
                          "on_chip": {"what": "SURVEY 8d second figure: per-iteration working set W_iter = 944 N bytes streamed at the measured "
                                              "ADMM iteration rate; the state is SM-resident, so this is ON-CHIP traffic-equivalent, NOT HBM",
                                      "w_iter_bytes": int(w_iter_bytes(mean_n)), "iterations_per_s": it_per_s,
                                      "equivalent_GBps": it_per_s * w_iter_bytes(mean_n) / 1e9,
                                      "vs_hbm_peak": it_per_s * w_iter_bytes(mean_n) / 1e9 / peak},
-                         "units": prof.get("units"),
                          "note": "state is SM-resident by design: compulsory HBM traffic is I/O only (SURVEY 8d); the kernel is bound by "
-                                 "dependent-issue latency and the shared-memory pipe, see profiles/"},
+                                 "dependent-issue latency and the shared-memory pipe (DESIGN.md)"},
             "clocks": clocks, "solved_fraction": n_solved / n_paths, "wall_ms_per_step": wall_ms / steps,
             "iters_per_solve_mean": iters_mean, "iters_per_solve_max": int(r["iters"].max()),
             "per_rank": {"solve_kernel_ms": [float(x) for x in all_ranks[:, 0]], "allgather_ms": [float(x) for x in all_ranks[:, 1]],
@@ -727,6 +775,8 @@ def main():
                     help="type string of OsqpSolver::create to solve the config with (default KP: the BASELINE metric)")
     ap.add_argument("--cpu-threads", type=int, default=0, help="CPU arm thread count (default: physical cores)")
     ap.add_argument("--no-extras", action="store_true", help="skip the config 3/4/5 context measurements of the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (rank 0's shard) as DIR/<name>.npy, float64, at most 64 MB in all")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * pqp.h -- C ABI of the B200-native batched path-QP solver ("pqp").
+ * pqp.h -- C ABI of the H100-native batched path-QP solver ("pqp").
  *
  * This is the drop-in boundary for the ONE hot path of LiJiangnanBit/path_optimizer:
  *   OsqpSolver::create(type, reference_path, vehicle_state, horizon)->solve(&path)
@@ -269,14 +269,14 @@ int pqp_solve_batch_device_classes(pqp_handle *h, int formulation, int batch, in
 /* Launch-order hint for the next solves of a batch of `batch` paths: expected ADMM iterations per path, e.g. the
  * `iters` the previous planning cycle reported for the same candidates.  Inside a kernel class the paths are then
  * launched longest expected work (stations x iterations) first instead of longest path first, which shortens the tail of
- * a launch whose paths outnumber the resident CTA slots only a few times (1024 paths on one B200: 23 % of the launch is
- * tail, an exact hint recovers about half of it; DESIGN.md section 6).  Results do not depend on the order.  NULL or batch 0 clears
+ * a launch whose paths outnumber the resident CTA slots only a few times (1024 x 100 on one H100: 5.16 ms in index order,
+ * 4.43 ms with an exact hint; DESIGN.md section 6).  Results do not depend on the order.  NULL or batch 0 clears
  * the hint; a hint whose length differs from a call's batch is ignored by that call.  No reference counterpart. */
 int pqp_set_order_hint(pqp_handle *h, int batch, const int32_t *expected_iters);
 
 const char *pqp_last_error(void);
 
-/* "pqp <abi> sm_100a <build info>" */
+/* "pqp <abi> sm_90a <build info>" */
 const char *pqp_version(void);
 
 /* Largest n_points a path may have on this device (one path must fit one SM's shared memory; longer paths report
@@ -291,7 +291,7 @@ int pqp_max_points_keep(pqp_handle *h, int formulation, int keep);
  * (n_points, keep) as pqp_solve_batch / pqp_solve_batch_device_classes / pqp_plan_batch choose it -- index into the
  * class table (order of preference), CTA size and dynamic shared memory; PQP_ERR_UNSUPPORTED when no class takes the
  * path (it would report PQP_INVALID_PROBLEM).  pqp_device_class_info: the single class pqp_solve_batch_device picks for
- * the caller's bounds.  smem_optin = the device's opt-in shared memory per block (0: B200's 232448). */
+ * the caller's bounds.  smem_optin = the device's opt-in shared memory per block (0: H100's 232448). */
 int pqp_class_info(int n_points, int keep, int smem_optin, int *variant, int *threads, int64_t *smem_bytes);
 int pqp_class_info_kpc(int n_points, int smem_optin, int *variant, int *threads, int64_t *smem_bytes);   /* the same for a "KPC" path (keep_control_steps is 4); PQP_ERR_UNSUPPORTED: longer than the largest KPC class (256 stations) */
 int pqp_class_info_form(int formulation, int n_points, int keep, int smem_optin, int *variant, int *threads, int64_t *smem_bytes);   /* any formulation ("K": keep ignored) */

@@ -32,7 +32,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -m path_optimizer_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback.")
+            "(nvcc, sm_90a).  There is no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp = C.c_void_p
     L.pqp_params_default.argtypes = [C.POINTER(Params)]

@@ -1,4 +1,4 @@
-"""Builds libpqp.so (the C-ABI shared library with the sm_100a kernels) in-tree with nvcc.
+"""Builds libpqp.so (the C-ABI shared library with the sm_90a kernels) in-tree with nvcc.
 
 Every .cu under csrc/ is compiled to its own object (in parallel) and the objects are linked into one shared
 library: each solve kernel sits in its own translation unit on purpose (csrc/pqp_kernels.h)."""
@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.environ.get("PQP_LIB_OUT") or os.path.join(_HERE, "libpqp.so")   # PQP_LIB_OUT / PQP_NVCC_EXTRA: A/B builds (diagnostics)
 OBJ = os.path.join(_HERE, "_obj" + os.environ.get("PQP_OBJ_SUFFIX", ""))
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-diag-suppress", "550,177"]
 
 
@@ -30,7 +30,7 @@ def is_stale():
 
 
 def build(force=False, verbose=False, jobs=None):
-    """Compile every .cu under csrc/ for sm_100a and link path_optimizer_b200/libpqp.so."""
+    """Compile every .cu under csrc/ for sm_90a and link path_optimizer_b200/libpqp.so."""
     if not force and not is_stale():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "nvcc")
@@ -53,7 +53,7 @@ def build(force=False, verbose=False, jobs=None):
         for _, log in results:
             print(log, end="")
     objs = [o for o, _ in results]
-    subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs + ["-ldl"], check=True)
+    subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs + ["-ldl"], check=True)
     return LIB_PATH
 
 

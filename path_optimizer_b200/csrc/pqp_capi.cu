@@ -1,5 +1,5 @@
 // pqp_capi.cu -- extern "C" boundary of libpqp.so (declared in include/pqp.h) and the kernel
-// launchers.  Host orchestration only: all numerics run in the sm_100a kernels; there is no CPU
+// launchers.  Host orchestration only: all numerics run in the sm_90a kernels; there is no CPU
 // fallback (pqp_create fails when no CUDA device / kernel image is usable).
 #include <cuda_runtime.h>
 #include <math.h>
@@ -274,7 +274,7 @@ extern "C" {
 
 const char *pqp_last_error(void) { return g_err; }
 
-const char *pqp_version(void) { return "pqp abi 1 / sm_100a / fp64 ADMM, one CTA per path (thread per station)"; }
+const char *pqp_version(void) { return "pqp abi 1 / sm_90a / fp64 ADMM, one CTA per path (thread per station)"; }
 
 int pqp_params_update_config(pqp_params *p) {
     if (!p) return PQP_ERR_ARG;
@@ -411,7 +411,7 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
     PQP_TRY(cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
     PQP_TRY(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, device));
     pqp_k1_set_smem_cap(h->smem_optin);
-    // fails with cudaErrorNoKernelImageForDevice / InvalidDeviceFunction on anything but sm_100
+    // fails with cudaErrorNoKernelImageForDevice / InvalidDeviceFunction on anything but sm_90
     for (int v = 0; v < kNumVariants; ++v)
         PQP_TRY(cudaFuncSetAttribute(kVariants[v].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     PQP_TRY(cudaFuncSetAttribute(pqp_gen_kernel_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));

@@ -1,4 +1,4 @@
-// pqp_device.cuh -- shared definitions for the batched path-QP kernels (sm_100a).
+// pqp_device.cuh -- shared definitions for the batched path-QP kernels (sm_90a).
 //
 // Hot path being replaced: OsqpSolver::solve() of LiJiangnanBit/path_optimizer
 // (reference src/solver/solver.cpp:46-77): QP assembly (solver_kp_as_input.cpp:45-203), the
@@ -93,7 +93,7 @@ PQP_DEV double limit_scaling(double v) {
 
 PQP_DEV double clampd(double v, double lo, double hi) { return fmin(fmax(v, lo), hi); }
 // Same projection for lo <= hi, with the two compares independent of each other (a dependent
-// fmin(fmax()) on doubles costs ~50 cycles on sm_100: DSETP + SEL + SEL, twice).
+// fmin(fmax()) on doubles costs ~50 cycles on sm_90: DSETP + SEL + SEL, twice).
 PQP_DEV double clamp2(double v, double lo, double hi) {
     double z = v;
     z = (v < lo) ? lo : z;

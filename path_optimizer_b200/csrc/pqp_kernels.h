@@ -1,7 +1,7 @@
 // pqp_kernels.h -- one record per compiled solve kernel ("shape class").  Every kernel lives in its own
 // translation unit (pqp_k*.cu): at the 255-register limit ptxas' allocation for one kernel changes with whatever
-// else is compiled next to it (measured: the same source ran 3x slower after unrelated instantiations were added to
-// the same file), so the kernels are compiled in isolation and only these records cross the boundary.
+// else is compiled next to it (the same source has run several times slower after unrelated instantiations were added
+// to the same file), so the kernels are compiled in isolation and only these records cross the boundary.
 #pragma once
 #include <stddef.h>
 

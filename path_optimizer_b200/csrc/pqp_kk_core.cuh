@@ -30,7 +30,7 @@
 #include "pqp_kp_core.cuh"
 
 #ifndef PQP_KK_G_SMEM
-#define PQP_KK_G_SMEM 0     // 1: G_L / G_R are read from their shared-memory rows in every solve instead of living in registers (measured slower: 13.5 vs 12.0 ms per 1024 x 100)
+#define PQP_KK_G_SMEM 0     // 1: G_L / G_R are read from their shared-memory rows in every solve instead of living in registers (slower: more shared-memory traffic on the solve's critical path)
 #endif
 
 namespace pqp {

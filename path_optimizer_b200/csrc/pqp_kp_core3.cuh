@@ -66,7 +66,7 @@ struct Kp3 {
     // of the CTA instead of M serial banded substitutions on warp 0 (the longest phase of an iteration).
     // Two-level separator system (every 34-separator class): the odd separators of the block-tridiagonal Schur system
     // are eliminated in closed form (3x3 blocks), only the even ones keep a dense inverse (<= 51 x 51 instead of
-    // 102 x 102: N = 200 runs 13.2 ms per 1024 paths instead of 22.2 ms).
+    // 102 x 102: a quarter of the shared memory and of the separator product's work).
     static constexpr bool kTwoLevel = (MMAX > 17);
     static constexpr bool kDense = (IMAX <= 17);   // (17-unknown interiors: 2 x 95 KB at 17 separators, 181 KB at 34 -- one CTA per SM either way)
     static constexpr int kSolveT = (MMAX + 31) / 32 * 32;   // threads that run the banded interior solves (non-dense form)
@@ -1051,9 +1051,8 @@ struct Kp3 {
             const int yQ = IMAX * M;
             // Phase (b2) of the dense form.  The separator product x_S = Sinv g runs on the first nSr threads, the row tasks
             // of y = K_I^-1 r_I on the WARPS after them: a warp that held both kinds of thread would run the two pieces of
-            // work one after the other and become the slowest of the phase (4.40 -> 4.10 ms per 1024 x 100).  (Handing the
-            // last, partly filled round of row tasks to the product warps, or two row tasks per loop trip, measured
-            // 1-4 % slower: profiles/r02_experiments.md.)
+            // work one after the other and become the slowest of the phase.  (Handing the last, partly filled round of row
+            // tasks to the product warps, or two row tasks per loop trip, were slower.)
             const int yT0 = (nSr + 31) & ~31, yNw = kT - yT0;
 #ifdef PQP_PHASE_TIMING
             static_assert(!kScratchOnVec, "phase timing uses exchange row 5, which the long-path classes give to the separator rhs");
@@ -1306,7 +1305,7 @@ struct Kp3 {
                     tu = PQP_TX(ub.pos);
                 }
 #undef PQP_TX
-                // (publishing x-tilde into a vector of its own saves this barrier and measured 7 % SLOWER: 4.10 -> 4.39 ms)
+                // (publishing x-tilde into a vector of its own saves this barrier but was SLOWER)
                 c.sync();   // everyone has consumed tr (rhs): publish x-tilde there for the neighbours
                 if (st.live) { s.tr()[st.pos] = ta; s.tr()[st.pos + 1] = tb; s.tr()[st.pos + 2] = tc; }
                 if (ub.live) s.tr()[ub.pos] = tu;

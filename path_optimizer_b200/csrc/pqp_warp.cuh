@@ -1,6 +1,6 @@
 // pqp_warp.cuh -- the warp abstraction the solver core is written against.
 //
-// Product build (nvcc, sm_100a): `Warp` maps 1:1 onto hardware intrinsics (__shfl_sync,
+// Product build (nvcc, sm_90a): `Warp` maps 1:1 onto hardware intrinsics (__shfl_sync,
 // __syncwarp); everything inlines away.
 //
 // Test-only build (-DPQP_HOST_EMU, plain g++): `Warp` is backed by 32 host threads and a barrier so

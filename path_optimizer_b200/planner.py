@@ -8,7 +8,7 @@ Reference interfaces being mirrored:
   PathOptimizer::solveWithoutSmoothing                   src/path_optimizer/path_optimizer.cpp:87-117
   tk::spline set_points / operator() / deriv             src/tools/spline.cpp:161-318
 
-All numerics run in libpqp.so's sm_100a kernels (spline_fit / spline_eval are host helpers of the
+All numerics run in libpqp.so's sm_90a kernels (spline_fit / spline_eval are host helpers of the
 same library); this module only marshals buffers.
 """
 import ctypes as C

@@ -6,7 +6,7 @@ Reference interface being mirrored (names, argument meaning, error behaviour):
 `create` returns None (and logs) for an unknown type string exactly like the reference returns
 nullptr; `solve` returns False whenever OSQP's status would not be SOLVED (osqp-eigen semantics).
 
-All numerics run in libpqp.so's sm_100a kernels; this module only marshals buffers.
+All numerics run in libpqp.so's sm_90a kernels; this module only marshals buffers.
 """
 import ctypes as C
 import logging

@@ -1,4 +1,5 @@
-// Latency micro-benchmarks for the primitives the path-QP kernel is built from (sm_100a, B200).
+// Latency micro-benchmarks for the primitives the path-QP kernel is built from (sm_90a, H100).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o profiles/micro/lat profiles/micro/lat.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define N_IT 4096
@@ -95,8 +96,10 @@ int main() {
     k_lds<<<1, 32, 4096 * 8>>>(out, cyc);
     k_bar<<<1, 128>>>(out, cyc);
     cudaFuncSetAttribute(k_local, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024);
-    k_local<<<296, 128, 110 * 1024>>>(out, cyc, 5);
-    k_dfma_tp<<<148, 512>>>(out, cyc, 0.999, 0.001);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    k_local<<<2 * sms, 128, 110 * 1024>>>(out, cyc, 5);
+    k_dfma_tp<<<sms, 512>>>(out, cyc, 0.999, 0.001);
     long long h[8];
     cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
     printf("dependent DFMA        : %.2f cycles/op\n", (double)h[0] / N_IT);

@@ -1,5 +1,5 @@
 import os, sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 from path_optimizer_b200 import synth
 from path_optimizer_b200.solver import BatchPathSolver
 b = synth.curvy_corridors(1024, 100)

@@ -1,7 +1,7 @@
 """ctypes loader for the CPU warp-emulator build of the product's solver source (TEST HARNESS).
 
 Builds tests/emu/libkp_emu.so from tests/emu/kp_emu.cpp with plain g++ (-DPQP_HOST_EMU) and runs
-the SAME pqp_kp_core.cuh that nvcc compiles for sm_100a, one host thread per lane.  Used by the
+the SAME pqp_kp_core.cuh that nvcc compiles for sm_90a, one host thread per lane.  Used by the
 CPU test-suite to check the kernel logic against the oracle without a GPU; never used by the product.
 """
 import ctypes as C

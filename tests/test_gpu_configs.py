@@ -1,4 +1,4 @@
-"""GPU tests of BASELINE configs 3, 4, 5 AT THEIR NAMED PER-GPU SIZES (run with -m gpu on the B200 box): the whole
+"""GPU tests of BASELINE configs 3, 4, 5 AT THEIR NAMED PER-GPU SIZES (run with -m gpu on an H100): the whole
 shard is solved through the C ABI, a >= 64-path sample of it is compared with the oracle (identical status, identical
 ADMM iteration count, 1e-8 on the Frenet and Cartesian states), and the device-resident entry points are checked
 against the host-buffer one bit for bit."""

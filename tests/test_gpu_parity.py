@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI
 (libpqp.so), against the CPU oracle on the same seeded inputs, against the committed golden fixtures,
 and -- at BASELINE.json's full sizes -- through size-independent properties.
 
