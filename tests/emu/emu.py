@@ -47,10 +47,32 @@ def lib():
     return _lib
 
 
+# The emulator's variant of every kernel class the library compiles, by the name pqp_class_name reports for it: tests
+# take the class from the library's own selection (tests/shapes.py) and run that class here.
+VARIANTS = {
+    "pqp_kp_solve_kernel": 0,
+    "pqp_kp3_solve_kernel<17,6,4,17>": 5,
+    "pqp_kp3_solve_kernel<23,7,4,17>": 6,
+    "pqp_kp3_solve_kernel<27,7,8,34>": 7,
+    "pqp_kp3_solve_kernel<17,6,8,34>": 8,
+    "pqp_kp3_solve_kernel<23,7,8,34>": 9,
+    "pqp_kp3_solve_kernel<37,7,13,34>": 10,
+    "pqp_kp3_solve_kernel<37,7,12,34>": 11,
+    "pqp_kp3_solve_kernel<27,7,10,34>": 12,
+    "pqp_kp3_solve_kernel<23,7,4,17,KPC>": 20,
+    "pqp_kp3_solve_kernel<23,7,8,34,KPC>": 21,
+    "pqp_kp3_solve_kernel<13,7,8,34,KPC>": 22,
+    "pqp_kk_solve_kernel<4>": 30,
+    "pqp_kk_solve_kernel<8>": 31,
+    "pqp_kk_solve_kernel<13>": 32,
+}
+
+
 def solve_batch(params, batch, smem_bytes=227 * 1024, variant=0, nwarps=4, max_k=None, max_kp=None):
-    """variant 0 = one-warp generic core (pqp_kp_core.cuh); 5..7 = Kp3<17,6,4>, <23,7,4>, <27,7,8>; 8, 9 = the 34-separator eight-warp classes Kp3<17,6,8,34>, <23,7,8,34>;
-    10, 11, 12 = the long-path classes Kp3<37,7,13,34>, <37,7,12,34>, <27,7,10,34>;
-    20, 21 = the "KPC" classes Kp3<23,7,4,17,KPC>, <23,7,8,34,KPC> (need max_k / max_kp)."""
+    """`variant`: a value of VARIANTS (0 = the one-warp generic core, pqp_kp_core.cuh) or a class name.  KPC classes
+    need max_k / max_kp."""
+    if isinstance(variant, str):
+        variant = VARIANTS[variant]
     B = len(batch["n_points"])
     total = int(batch["offsets"][-1])
     ref = np.ascontiguousarray(batch["ref"], dtype=STATE_DTYPE)

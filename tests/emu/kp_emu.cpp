@@ -20,19 +20,21 @@ struct LaneArgs {
     int prob;
     double *smem;
     size_t smem_doubles;
-    int variant;  // 0: one-warp generic core; 5..11: thread-per-station classes (tests/emu/emu.py)
+    int variant;  // 0: one-warp generic core; 5..: thread-per-station classes (tests/emu/emu.py: VARIANTS)
 };
 void *lane_main(void *p) {
     LaneArgs *a = (LaneArgs *)p;
     pqp::Warp w{a->lane, a->sh};
     pqp::Cta c{w, pqp::CtaSync{a->cta}, a->wid, a->nw, a->smem};
-    const int res = a->nw > 8 ? 256 : 128;     // leading doubles: CTA reduction scratch (16 per warp)
+    // leading doubles: CTA reduction scratch (16 per warp) of the thread-per-station kernels (kCtaScratch); the one-warp
+    // kernel gets the whole allocation (pqp_k1_generic.cu), which its longest paths need
+    const int res = a->variant == 0 ? 0 : a->nw > 8 ? 256 : 128;
     double *sm = a->smem + res;
     const size_t cap = a->smem_doubles - res;
     switch (a->variant) {
     case 5: pqp::Kp3<17, 6, 4>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
     case 6: pqp::Kp3<23, 7, 4>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
-    case 7: pqp::Kp3<27, 7, 8>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
+    case 7: pqp::Kp3<27, 7, 8, 34>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
     case 8: pqp::Kp3<17, 6, 8, 34>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
     case 9: pqp::Kp3<23, 7, 8, 34>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;
     case 10: pqp::Kp3<37, 7, 13, 34>::solve_path(c, *a->prm, *a->bv, a->prob, sm, cap); break;

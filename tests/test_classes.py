@@ -17,7 +17,7 @@ def _class(n, keep):
 
 def test_every_baseline_length_runs_thread_per_station():
     """Configs 2-5 use 0.3 m stations (keep_control_steps 3) and 50..400 stations: none of them may fall back to the
-    chunked or one-warp kernels."""
+    one-warp kernel."""
     for keep in (3, 4):
         for n in range(2, 409):
             rc, name, threads, smem = _class(n, keep)
@@ -46,6 +46,23 @@ def test_device_class_covers_its_bounds(hint):
     assert L.pqp_device_class_info(hint[0], hint[1], hint[2], 0, C.byref(v), C.byref(t), C.byref(s)) == 0
     assert t.value >= hint[0] or t.value == 32
     assert s.value <= 232448
+
+
+def test_shape_sweeps_reach_every_class():
+    """The GPU shape sweep (test_gpu_shapes.py) runs every length at the keep values of its station spacings: together
+    they reach every class each formulation selects, and every compiled class is either selected or listed as not
+    selected.  The emulator runs each compiled class under the name the library reports for it."""
+    from tests import shapes
+    from tests.emu import emu
+    assert shapes.kp_keeps() == [1, 2, 3, 4, 5, 7, 8, 10]
+    for form, keeps in ((shapes.KP, shapes.kp_keeps()), (shapes.K, [1]), (shapes.KPC, [4])):
+        reached = set()
+        for keep in keeps:
+            reached |= set(shapes.class_ranges(form, keep))
+        assert reached == set(shapes.CLASSES[form]), (form, sorted(reached ^ set(shapes.CLASSES[form])))
+    compiled = shapes.compiled_classes()
+    assert sorted(compiled) == sorted(sum(shapes.CLASSES.values(), []) + shapes.UNSELECTED)
+    assert set(emu.VARIANTS) == set(compiled)
 
 
 def test_device_class_refuses_bounds_no_single_class_takes():

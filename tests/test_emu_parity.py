@@ -2,31 +2,28 @@
 under a 32-thread warp emulator (tests/emu) and compared with the oracle.  This checks the
 matrix-free scaling, the partitioned banded KKT solve, the ADMM recurrence, termination and adaptive
 rho without a GPU.  The emulator is a test harness only; the product has no CPU path."""
+import re
+
 import numpy as np
 import pytest
 
 from oracle import oracle
 from path_optimizer_b200 import synth
+from tests import shapes
 from tests.emu import emu
 
 TOL = 1e-9  # same recurrence in fp64: agreement is ~1e-13 in practice
 
 
 def _variant_for(batch):
-    """One emulator variant for the whole batch: the class the library would pick (pick_variant in pqp_capi.cu) when
-    every path maps onto the same one, else a class wide enough for all of them."""
-    keeps = [oracle.keep_control_steps(0, batch["ref"][batch["offsets"][b]:batch["offsets"][b + 1]])
-             for b in range(len(batch["n_points"]))]
-    nmax, kmax = int(batch["n_points"].max()), max(keeps)
-    if kmax > 4:
-        return 0          # one-warp generic kernel
-    if kmax <= 3 and nmax <= 102:
-        return 5          # Kp3<17,6,4>  (thread-per-station production kernel)
-    if nmax <= 128 and min(keeps) == 4:
-        return 6          # Kp3<23,7,4>
-    if nmax <= 153:
-        return 7          # Kp3<27,7,8> (17 separators): keep 1..4
-    return 0
+    """One emulator variant for the whole batch, from the library's own selection: the class pqp_solve_batch launches
+    when every path maps onto the same one, else the one class pqp_solve_batch_device takes for all of them."""
+    o = batch["offsets"]
+    keeps = [shapes.keep_of(shapes.KP, batch["ref"][o[b]:o[b + 1]]) for b in range(len(batch["n_points"]))]
+    names = {shapes.class_of(shapes.KP, n, k)[0] for n, k in zip(batch["n_points"], keeps)}
+    if len(names) > 1:
+        names = {shapes.device_class_of(int(batch["n_points"].max()), min(keeps), max(keeps))}
+    return emu.VARIANTS[names.pop()]
 
 
 def _check(batch, params, variant=None):
@@ -91,10 +88,78 @@ def test_emu_generic_core_still_matches(oracle_params):
                                            (10, 257, 0.3), (10, 408, 0.25), (11, 384, 0.3), (12, 300, 0.3),   # thirteen- / twelve- / ten-warp long-path classes
                                            (0, 400, 0.3)])   # one-warp kernel with its scalings in the global workspace
 def test_emu_shape_classes(oracle_params, variant, n, ds):
+    """One full-length solve on a given class (emu.VARIANTS) at a length it takes.  Mostly the class the library selects
+    for the path; 7 (Kp3<27,7,8,34>, selected for 205..256 stations at keep 3) at 128 / 150 and the one-warp kernel at
+    400 stations run a class's source at lengths the selection gives to another class.
+    test_emu_selected_classes runs the selected class."""
     b = synth.curvy_corridors(1, n)
     if ds != 0.3:
         b["ref"]["s"] = np.arange(n) * ds
     _check(b, oracle_params, variant=variant)
+
+
+@pytest.mark.parametrize("n", [205, 256, 414])
+def test_emu_selected_classes(oracle_params, n):
+    """One full-length solve on the class the library selects for the path (0.3 m accumulated: keep 3):
+    Kp3<27,7,8,34> at both ends of its range, and the one-warp kernel at its longest path (414 stations), which needs
+    the whole shared-memory allocation."""
+    _check(synth.curvy_corridors(1, n), oracle_params)
+
+
+# station spacing (accumulated) per keep value: int(1.2 / ds) == keep for every path length, 2 stations included
+EDGE_SPACING = {1: 1.0, 2: 0.5, 3: 0.35, 4: 0.28}
+
+
+def _edge_lengths(form, keep, name, lo, hi):
+    m = re.fullmatch(r"pqp_kp3_solve_kernel<\d+,\d+,\d+,(\d+)(,KPC)?>", name)
+    if m:
+        return shapes.partition_edges(lo, hi, lambda n: shapes.kp3_partition(n, keep, int(m.group(1))))
+    m = re.fullmatch(r"pqp_kk_solve_kernel<([48])>", name)      # SPIKE form (the 13-warp class has no partition)
+    if m:
+        return shapes.partition_edges(lo, hi, lambda n: shapes.kk_partition(n, 26 if m.group(1) == "4" else 32))
+    return [lo, hi]
+
+
+@pytest.mark.parametrize("form,keep", [(0, 1), (0, 2), (0, 3), (0, 4), (2, 4), (1, 1)], ids=["KP1", "KP2", "KP3", "KP4", "KPC", "K"])
+def test_emu_partition_edges(oracle_params, form, keep):
+    """Every class the library selects for (formulation, keep), at the path lengths where its partition changes
+    (tests/shapes.py: partition_edges -- ends of the class, both sides of every change of the separator spacing, first
+    and last new separator at each spacing, odd and even separator counts), run on that class under the emulator and
+    compared with the oracle.  max_iter = 50: both sides stop there, after the rho updates and termination checks on
+    the way; the full-length runs are the GPU shape sweep (test_gpu_shapes.py)."""
+    p = oracle_params.copy()
+    p.max_iter = 50
+    n_points, names = [], []
+    for name, (lo, hi) in sorted(shapes.class_ranges(form, keep).items(), key=lambda kv: kv[1]):
+        edges = _edge_lengths(form, keep, name, lo, hi)
+        n_points += edges
+        names += [name] * len(edges)
+    b = synth.curvy_corridors(len(n_points), n_points=n_points)
+    o = b["offsets"]
+    ds = EDGE_SPACING.get(keep, 0.3)
+    for i, n in enumerate(n_points):
+        b["ref"]["s"][o[i]:o[i + 1]] = synth._accumulate_s(n, ds)
+        assert shapes.keep_of(form, b["ref"][o[i]:o[i + 1]]) == keep
+        assert shapes.class_of(form, n, keep) == (names[i], True)
+    mk = mkp = None
+    if form == shapes.KPC:
+        b["ref"]["v"] = 4.0 + 3.0 * np.sin(np.arange(o[-1]) * 0.05)
+        b["ref"]["a"] = 0.5 * np.cos(np.arange(o[-1]) * 0.05)
+        b["ref"]["v"][::11] = 0.0
+        mk, mkp = oracle.update_limits(oracle_params, b["ref"])
+    ref = oracle.solve_batch(p, form, b, threads=8, max_k=mk, max_kp=mkp)
+    names = np.array(names)
+    for name in dict.fromkeys(names):
+        idx = np.nonzero(names == name)[0]
+        sub = synth.take_paths(b, idx)
+        sel = np.concatenate([np.arange(o[i], o[i + 1]) for i in idx])
+        e = emu.solve_batch(p, sub, variant=name, max_k=None if mk is None else mk[sel], max_kp=None if mk is None else mkp[sel])
+        bad = (e["status"] != ref["status"][idx]) | (e["iters"] != ref["iters"][idx])
+        assert not bad.any(), (name, "N =", np.asarray(n_points)[idx][bad].tolist())
+        for f in range(3):
+            np.testing.assert_allclose(e["frenet"][:, f], ref["frenet"][sel, f], rtol=0, atol=TOL, err_msg=name)
+        for f in "xyzks":
+            np.testing.assert_allclose(e["states"][f], ref["states"][f][sel], rtol=0, atol=TOL, err_msg=name)
 
 
 def _limits(batch):
@@ -126,15 +191,19 @@ def test_emu_generic_kernel_k_and_kpc(oracle_params, form):
 @pytest.mark.parametrize("variant", [0, 5, 7])
 def test_emu_primal_infeasible(oracle_params, variant):
     """Corridors with no feasible path: OSQP's primal-infeasibility certificate fires (status -3) at the
-    same check iteration as in the oracle, the output is NaN, feasible neighbours are untouched."""
-    b = synth.infeasible_corridors(6 if variant == 0 else 2, 60)
+    same check iteration as in the oracle, the output is NaN, feasible neighbours are untouched.  Kp3<17,6,4,17> (5)
+    and Kp3<27,7,8,34> (7) at lengths the library selects them for; the one-warp kernel (0) forced at 60 stations."""
+    n = 220 if variant == 7 else 60
+    b = synth.infeasible_corridors(6 if variant == 0 else 2, n)
+    if variant != 0:
+        assert emu.VARIANTS[shapes.class_of(shapes.KP, n, 3)[0]] == variant
     e = emu.solve_batch(oracle_params, b, variant=variant)
     o = oracle.solve_batch(oracle_params, 0, b)
     assert np.array_equal(e["status"], o["status"]) and np.array_equal(e["iters"], o["iters"])
     assert (o["status"][0::2] == -3).all() and (o["status"][1::2] == 1).all()
     assert (o["iters"][0::2] < 4000).all()
-    assert np.isnan(e["frenet"][:60]).all()
-    ok = np.repeat(o["status"] == 1, 60)
+    assert np.isnan(e["frenet"][:n]).all()
+    ok = np.repeat(o["status"] == 1, n)
     np.testing.assert_allclose(e["frenet"][ok], o["frenet"][ok], rtol=0, atol=TOL)
 
 

@@ -15,6 +15,7 @@ import pytest
 from oracle import oracle
 from path_optimizer_b200 import synth
 from path_optimizer_b200.abi import SOLVED
+from tests import shapes
 
 pytestmark = pytest.mark.gpu
 
@@ -215,8 +216,9 @@ def test_k_and_kpc_formulations(solver, oracle_params, form, name):
 
 
 def test_primal_infeasible_corridors(solver):
-    """No feasible path: status -3 at the oracle's check iteration, NaN output, on every kernel class
-    (thread-per-station, chunked, generic fallback via a long keep), neighbours untouched."""
+    """No feasible path: status -3 at the oracle's check iteration, NaN output, neighbours untouched: on the four- and
+    eight-warp KP classes, on the one-warp kernel through a long keep (0.2 m stations: keep 5), and on "K"
+    (test_gpu_shapes.py::test_verdicts_on_every_class runs it on every class)."""
     prm = oracle.default_params()
     for n, ds in ((60, 0.3), (180, 0.3), (60, 0.2)):
         b = synth.infeasible_corridors(16, n)
@@ -288,14 +290,37 @@ PARAM_CASES = {
     "maxiter60": dict(max_iter=60),
     "check0": dict(check_termination=0, max_iter=120),
     "vehicle": dict(car_length=4.2, car_width=1.8, rear_axle_to_center=1.2, wheel_base=2.6, max_steering_angle=0.45),
+    "k_weights": dict(K_curvature_weight=7.0, K_curvature_rate_weight=60.0, K_deviation_weight=0.4),
 }
+# accumulated station spacing per KP keep value: int(1.2 / ds) == keep for every path length, 2 stations included
+PARAM_SPACING = {3: 0.35, 4: 0.25, 5: 0.2}
+
+
+def _class_ends_batch(form):
+    """One path at the first and one at the last length of every class the formulation selects (KP: at keep 3 and 4,
+    and the one-warp kernel at keep 5; tests/shapes.py)."""
+    keeps = (3, 4, 5) if form == 0 else (4,) if form == 2 else (1,)
+    n_points, spacing = [], []
+    for keep in keeps:
+        for name, (lo, hi) in shapes.class_ranges(form, keep).items():
+            if keep < 5 or name == shapes.GENERIC:
+                n_points += [lo, hi]
+                spacing += [PARAM_SPACING.get(keep, 0.3)] * 2
+    b = synth.curvy_corridors(len(n_points), n_points=n_points)
+    o = b["offsets"]
+    for i, n in enumerate(n_points):
+        b["ref"]["s"][o[i]:o[i + 1]] = synth._accumulate_s(n, spacing[i])
+    got = {shapes.class_of(form, n, shapes.keep_of(form, b["ref"][o[i]:o[i + 1]])) for i, n in enumerate(n_points)}
+    assert got == {(name, True) for k in keeps for name in shapes.class_ranges(form, k)}
+    return b
 
 
 @pytest.mark.parametrize("case", sorted(PARAM_CASES))
 def test_parameter_sweep(case):
-    """Every field of pqp_params is honoured the way the oracle honours it, on every KP kernel class (thread-per-station,
-    chunked, generic fallback) and on the generic K kernel: intervals, tolerances, relaxation, weights, scaling,
-    end-heading switch, vehicle geometry (d1..d4 recomputed by pqp_params_update_config)."""
+    """Every field of pqp_params is honoured the way the oracle honours it, on every kernel class of every formulation
+    at both ends of its length range (KP at keep 3 and 4 and the one-warp kernel at keep 5, K, KPC): intervals,
+    tolerances, relaxation, weights, scaling, end-heading switch, vehicle geometry (d1..d4 recomputed by
+    pqp_params_update_config)."""
     import ctypes as C
     from path_optimizer_b200 import _lib
     from path_optimizer_b200.solver import BatchPathSolver
@@ -303,10 +328,10 @@ def test_parameter_sweep(case):
     for k, v in PARAM_CASES[case].items():
         setattr(p, k, v)
     _lib.load().pqp_params_update_config(C.byref(p))
-    s = BatchPathSolver(params=p, max_batch=16, max_total_points=16 * 300)
+    s = BatchPathSolver(params=p, max_batch=64, max_total_points=16384)
     b = synth.curvy_corridors(6, n_points=[60, 100, 33, 150, 220, 48])
     off = b["offsets"]
-    b["ref"]["s"][off[5]:off[6]] = np.arange(48) * 0.2          # keep = 6 -> generic fallback kernel
+    b["ref"]["s"][off[5]:off[6]] = np.arange(48) * 0.2          # keep = 5 (int(1.2 / 0.2) = 5) -> one-warp kernel
     res = s.solve(b)
     ref = oracle.solve_batch(p, 0, b, threads=6)
     assert np.array_equal(res["status"], ref["status"]), (res["status"], ref["status"])
@@ -317,18 +342,32 @@ def test_parameter_sweep(case):
     ok_ = oracle.solve_batch(p, 1, small, threads=3)
     assert np.array_equal(rk["status"], ok_["status"]) and np.array_equal(rk["iters"], ok_["iters"])
     np.testing.assert_allclose(rk["frenet"], ok_["frenet"], rtol=0, atol=FRENET_TOL)
+    # both ends of every class (runs past 1000 iterations: 1e-6, see tests/shapes.py)
+    for form, name in ((0, "KP"), (1, "K"), (2, "KPC")):
+        b = _class_ends_batch(form)
+        mk = mkp = None
+        if form == 2:
+            total = int(b["offsets"][-1])
+            b["ref"]["v"] = 4.0 + 3.0 * np.sin(np.arange(total) * 0.05)
+            b["ref"]["a"] = 0.5 * np.cos(np.arange(total) * 0.05)
+            b["ref"]["v"][::13] = 0.0
+            mk, mkp = oracle.update_limits(p, b["ref"])
+        res = s.solve(b, name, max_k=mk, max_kp=mkp)
+        ref = oracle.solve_batch(p, form, b, threads=8, max_k=mk, max_kp=mkp)
+        shapes.assert_matches(res, ref, np.arange(len(b["n_points"])), np.arange(int(b["offsets"][-1])), b["n_points"],
+                              f"{case} {name}")
     s.close()
 
 
 def test_config5_mixed_lengths_up_to_400(solver, oracle_params):
-    """BASELINE config 5 shape: path lengths drawn from 50..400 stations.  Every length has a kernel class (4-warp and
-    8-warp thread-per-station classes up to 256, the one-warp kernel beyond -- with its scalings in the global
-    workspace above ~340 stations); shards of equal total station count (parallel.shard_by_work) give the same results
-    as the whole batch."""
+    """BASELINE config 5 shape: path lengths drawn from 50..400 stations.  Every length has a thread-per-station class
+    at keep 3 (4 warps to 102 stations, 8 warps to 204 and 256, 10 / 12 / 13 warps to 306 / 384 / 408): both sides of
+    each class edge, and the longest path of the last class, are in the batch.  Shards of equal total station count
+    (parallel.shard_by_work) give the same results as the whole batch."""
     from path_optimizer_b200 import parallel
     rng = np.random.default_rng(31)
     n_points = rng.integers(50, 401, size=48)
-    n_points[:4] = [400, 399, 344, 343]
+    n_points[:12] = [102, 103, 204, 205, 256, 257, 306, 307, 384, 385, 400, 408]
     b = synth.curvy_corridors(48, n_points=n_points)
     res = solver.solve(b)
     ref = oracle.solve_batch(oracle_params, 0, b, threads=8)
