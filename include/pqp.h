@@ -265,6 +265,33 @@ int pqp_solve_batch_device_classes(pqp_handle *h, int formulation, int batch, in
                                    void *stream,
                                    pqp_stats *stats);
 
+/* Device-resident solve of a MIXED-LENGTH batch whose station counts exist on the device only: the arguments of
+ * pqp_solve_batch_device, and every path runs on the kernel class pqp_solve_batch would choose for it, with the same
+ * results bit for bit.  A dispatch kernel reads d_n_points, computes keep_control_steps from d_ref exactly as
+ * pqp_keep_control_steps does, looks the class up in the table pqp_create built with the host's own selection and sorts
+ * the paths into per-class launch order (longest first); every class the bounds can reach is then launched on internal
+ * lanes forked from / joined into `stream`.  The bounds only narrow what is launched: `max_n_points` >= every
+ * n_points[b] and, for "KP", `min_keep` <= keep_control_steps <= `max_keep` (each 0 = unknown).  A path outside the
+ * stated bounds reports PQP_INVALID_PROBLEM (0 iterations, NaN states); `total_points` must be offsets[batch].
+ * Asynchronous on `stream`; no host synchronisation unless `stats` is non-NULL; no allocation: after one warm-up call
+ * the call can be captured into a CUDA graph.  One call in flight per handle.  pqp_set_order_hint is not applied (the
+ * order inside a class is longest path first).  No reference counterpart. */
+int pqp_solve_batch_device_dispatch(pqp_handle *h, int formulation, int batch, int total_points,
+                                    int max_n_points, int min_keep, int max_keep,
+                                    const int32_t *d_n_points, const int32_t *d_offsets,
+                                    const pqp_state *d_ref,
+                                    const pqp_station_bounds *d_bounds,
+                                    const double *d_x0,
+                                    const double *d_end_heading,
+                                    const double *d_max_k,
+                                    const double *d_max_kp,
+                                    pqp_state *d_out_states,
+                                    double *d_out_frenet,
+                                    int32_t *d_status,
+                                    int32_t *d_iters,
+                                    void *stream,
+                                    pqp_stats *stats);
+
 /* Last error text for this thread (CUDA error strings etc.); never NULL. */
 /* Launch-order hint for the next solves of a batch of `batch` paths: expected ADMM iterations per path, e.g. the
  * `iters` the previous planning cycle reported for the same candidates.  Inside a kernel class the paths are then
@@ -298,6 +325,11 @@ int pqp_class_info_form(int formulation, int n_points, int keep, int smem_optin,
 const char *pqp_class_name(int variant);   /* kernel name of a class-table index, as profilers print it ("" if out of range) */
 int pqp_device_class_info(int max_n_points, int min_keep, int max_keep, int smem_optin, int *variant, int *threads,
                           int64_t *smem_bytes);
+/* The class table the device dispatch looks paths up in (pqp_solve_batch_device_dispatch), built by the same selection
+ * as pqp_class_info_form: 11 rows (keep_control_steps 1..10, then keep > 10) of *ncols class indices each, entry
+ * [keep - 1][n_points]; the last column is one station past the longest path any class of the formulation takes and
+ * stands for every longer path.  table = NULL: only *ncols.  PQP_ERR_CAPACITY when `capacity` < 11 * *ncols. */
+int pqp_class_table(int formulation, int smem_optin, int8_t *table, int capacity, int *ncols);
 
 #ifdef __cplusplus
 } /* extern "C" */

@@ -142,6 +142,32 @@ int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_m
                    int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds,
                    pqp_stats *stats);
 
+/* The same planner iteration on DEVICE arrays of the handle's device, e.g. reference paths another CUDA stage produced:
+ * nothing crosses to the host.  Arguments as pqp_plan_batch, with these differences:
+ *   d_offsets          [batch+1] exclusive prefix of d_n_points; total_points = d_offsets[batch]
+ *   max_n_points       >= every n_points[b]: sizes the bounds grid and bounds the class dispatch (0: the longest path
+ *                      any kernel class of the formulation takes).  A longer path reports PQP_INVALID_PROBLEM unless
+ *                      blocking cut it within its first max_n_points stations.
+ *   d_knot_offsets     [batch+1] exclusive prefix of the knot counts (IMPROVED only), instead of n_knots
+ *   d_out_states .. d_out_bounds   the caller's device buffers (d_iters, d_out_bounds optional; d_status required)
+ * The QP step picks every path's kernel class on the device (as pqp_solve_batch_device_dispatch), so each path runs on
+ * the class pqp_plan_batch would choose and the results equal pqp_plan_batch's bit for bit.  "KPC" derives its limits
+ * on the device as pqp_plan_batch does; stations past a cut read as zeros (RAW).  Asynchronous on `stream` (NULL: the
+ * handle's stream); no host synchronisation unless `stats` is non-NULL (then only kernel_ms and kernel_launches are
+ * filled); no allocation once an earlier call on the handle has sized its buffers: make one warm-up call, then the call
+ * can be captured into a CUDA graph and replayed after new inputs are copied into the captured buffers.  One call in
+ * flight per handle.  pqp_set_order_hint is not applied.  No reference counterpart. */
+int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                          int total_points, int max_n_points,
+                          const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                          const int32_t *d_knot_offsets, const double *d_knots,
+                          const double *d_x_coef, const double *d_y_coef,
+                          const double *d_x0, const double *d_end_heading,
+                          double output_spacing, int collision_check, int max_out,
+                          pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok,
+                          int32_t *d_status, int32_t *d_iters, pqp_station_bounds *d_out_bounds,
+                          void *stream, pqp_stats *stats);
+
 #ifdef __cplusplus
 } /* extern "C" */
 #endif

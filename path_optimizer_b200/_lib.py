@@ -12,10 +12,11 @@ LIB_PATH = os.environ.get("PQP_LIB") or os.path.join(_HERE, "libpqp.so")   # PQP
 SYMBOLS = ["pqp_params_default", "pqp_params_update_config", "pqp_keep_control_steps", "pqp_problem_size",
            "pqp_create", "pqp_destroy", "pqp_set_params", "pqp_solve_batch", "pqp_solve_batch_device",
            "pqp_solve_batch_device_classes", "pqp_last_error", "pqp_version", "pqp_max_points", "pqp_max_points_keep",
-           "pqp_class_info", "pqp_class_info_kpc", "pqp_class_info_form", "pqp_set_order_hint", "pqp_class_name", "pqp_device_class_info"]
+           "pqp_class_info", "pqp_class_info_kpc", "pqp_class_info_form", "pqp_set_order_hint", "pqp_class_name", "pqp_device_class_info",
+           "pqp_solve_batch_device_dispatch", "pqp_class_table"]
 # ... and include/pqp_env.h
 ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "pqp_map_distance", "pqp_spline_fit", "pqp_spline_eval", "pqp_update_bounds_batch",
-               "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch"]
+               "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -57,6 +58,8 @@ def load():
     L.pqp_class_name.restype = C.c_char_p
     L.pqp_device_class_info.argtypes = [C.c_int] * 4 + [C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int64)]
     L.pqp_solve_batch_device_classes.argtypes = [vp] + [C.c_int] * 3 + [vp] * 15 + [C.POINTER(Stats)]
+    L.pqp_solve_batch_device_dispatch.argtypes = [vp] + [C.c_int] * 6 + [vp] * 13 + [C.POINTER(Stats)]
+    L.pqp_class_table.argtypes = [C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int)]
     # include/pqp_env.h
     L.pqp_update_limits.argtypes = [C.POINTER(Params), C.c_int, C.c_int, vp, vp, vp]
     L.pqp_update_limits_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp]
@@ -71,6 +74,8 @@ def load():
     L.pqp_densify_batch.argtypes = [vp, C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, vp, vp, C.POINTER(Stats)]
     L.pqp_plan_batch.argtypes = ([vp, C.c_int, C.c_int, C.c_int, C.c_int] + [vp] * 8 +
                                  [C.c_double, C.c_int, C.c_int] + [vp] * 6 + [C.POINTER(Stats)])
+    L.pqp_plan_batch_device.argtypes = ([vp] + [C.c_int] * 6 + [vp] * 9 + [C.c_double, C.c_int, C.c_int] + [vp] * 7 +
+                                        [C.POINTER(Stats)])
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

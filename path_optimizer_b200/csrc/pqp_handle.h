@@ -49,6 +49,22 @@ struct pqp_handle {
     // pqp_set_order_hint: expected ADMM iterations per path (e.g. the previous planning cycle's counts); launch order
     // inside a class becomes longest-expected-first
     std::vector<int32_t> order_hint;
+    // device dispatch (pqp_solve_batch_device_dispatch, pqp_plan_batch_device): the class table of every formulation
+    // (pqp_dispatch.h; rows x cls_ncols[form] entries at d_cls_table + cls_off[form]), per-class order segments
+    // (max classes of a formulation x max_batch), one sort key per path, and the station counts, status and iterations
+    // the dispatched launches see: max_batch + 1 entries, the last one a path of 0 stations for unused order entries
+    int8_t *d_cls_table = nullptr;
+    int cls_ncols[3] = {}, cls_off[3] = {};
+    int32_t *d_disp_order = nullptr, *d_disp_key = nullptr;
+    int32_t *d_disp_n = nullptr, *d_disp_status = nullptr, *d_disp_iters = nullptr;
+    // launches of the last bounds the dispatch was asked for (form, max_n, min_keep, max_keep as passed)
+    struct DispatchLaunches {
+        bool valid = false;
+        int form = 0, max_n = 0, min_keep = 0, max_keep = 0;
+        bool reach[PQP_MAX_VARIANTS] = {};
+        int min_n[PQP_MAX_VARIANTS] = {};
+        size_t smem[PQP_MAX_VARIANTS] = {};
+    } disp;
     // device buffers for the host-pointer entry point
     int32_t *d_n = nullptr, *d_off = nullptr, *d_order = nullptr, *d_status = nullptr, *d_iters = nullptr;
     int32_t *d_order_auto = nullptr;   // launch order computed on the device (pqp_solve_batch_device, small batches)
@@ -73,6 +89,14 @@ struct pqp_handle {
 // pqp_solve_batch_device_classes.
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
                           const pqp_state *ref, const int32_t *keep, cudaStream_t st, int *launches, int form = 0 /* PQP_FORM_KP; 2 = KPC (bv.max_k / max_kp set) */);
+
+// Internal (pqp_capi.cu): the same launches when the station counts exist on the device only.  A dispatch kernel reads
+// them, derives keep_control_steps from the device-side reference states, looks every path up in the class table and
+// sorts the paths into per-class order segments (longest first); every class the bounds can reach is launched over its
+// segment.  A path outside the bounds (max_n, min_keep..max_keep; 0 = unknown) reports PQP_INVALID_PROBLEM.
+// `total` = offsets[batch] bounds the grid of each class.  No host synchronisation, no allocation.
+int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
+                        int max_keep, cudaStream_t st, int *launches);
 
 // thread-local error text returned by pqp_last_error()
 extern thread_local char pqp_g_err[512];

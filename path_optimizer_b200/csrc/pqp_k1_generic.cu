@@ -14,7 +14,10 @@ pqp_kp_solve_kernel(const __grid_constant__ pqp::DevParams prm, const __grid_con
 }
 
 // Shared memory for a path: with the scalings on chip when that fits the 227 KB a CTA can opt into, else with the
-// scalings in the global workspace (the kernel makes the same choice from the size it is launched with).
+// scalings in the global workspace (the kernel makes the same choice from the size it is launched with).  The choice is
+// per path: a launch carries the largest need of the paths it may get, never more than the opt-in, so a path whose
+// on-chip layout fits the opt-in finds at least that much and one whose layout does not finds less.  A launch sized
+// for more paths (the device dispatch) cannot move a path's scalings.
 static size_t g_cap = 232448;   // opt-in shared memory per block of the device in use (H100: 227 KB); pqp_create passes the real value
 void pqp_k1_set_smem_cap(int bytes) { if (bytes > 0) g_cap = (size_t)bytes; }
 static size_t g_smem(int n, int keep) {

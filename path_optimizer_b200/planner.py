@@ -175,3 +175,47 @@ class PathPlanner(BatchPathSolver):
             raise PqpError(f"pqp_plan_batch failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, n_out=n_out, ok=ok, status=status, iters=iters, bounds=bounds,
                     solved=(status == SOLVED), stats=stats)
+
+    def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
+                    bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
+                    collision_check=True, max_out=512, want_bounds=False, out=None, stats=False):
+        """plan() on torch CUDA tensors of the planner's device (path_optimizer_b200.device): n_points int32 [B],
+        offsets int32 [B + 1], ref float64 [T, 7], x0 float64 [B, 3], end_heading float64 [B]; `splines` (IMPROVED)
+        a dict of knot_offsets int32 [B + 1], knots [K], x_coef / y_coef [K, 4] (device.splines_to_device).  The whole
+        chain runs on the device (pqp_plan_batch_device) on torch.cuda.current_stream() with plan()'s results bit for
+        bit and no host synchronisation (unless `stats`): after one warm-up call it can be captured in a CUDA graph.
+        max_n_points >= every n_points (0: the longest path any kernel class takes).  `out` may carry the output
+        tensors (states: [T, 7] RAW or [B, max_out, 7] DENSIFY; n_out, ok, status, iters; bounds [T, 8])."""
+        import torch
+        from . import device as D
+        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
+        dev = self._cuda_device()
+        B, T = int(n_points.shape[0]), int(ref.shape[0])
+        f64, i32 = torch.float64, torch.int32
+        out = dict(out or {})
+        shape = (T, D.STATE_COLS) if output_mode == OUTPUT_RAW else (B, int(max_out), D.STATE_COLS)
+
+        def buf(name, shp, dtype):
+            return out[name] if out.get(name) is not None else torch.empty(shp, dtype=dtype, device=dev)
+        states = buf("states", shape, f64)
+        n_out, ok, status, iters = buf("n_out", (B,), i32), buf("ok", (B,), i32), buf("status", (B,), i32), buf("iters", (B,), i32)
+        bounds = buf("bounds", (T, D.BOUNDS_COLS), f64) if want_bounds else None
+        spl = splines or {}
+        K = int(spl["knots"].shape[0]) if splines is not None else 0
+        args = [D.check(n_points, "n_points", i32, (B,), dev), D.check(offsets, "offsets", i32, (B + 1,), dev),
+                D.check(ref, "ref", f64, (T, D.STATE_COLS), dev),
+                D.check(spl.get("knot_offsets"), "knot_offsets", i32, (B + 1,), dev),
+                D.check(spl.get("knots"), "knots", f64, (K,), dev), D.check(spl.get("x_coef"), "x_coef", f64, (K, 4), dev),
+                D.check(spl.get("y_coef"), "y_coef", f64, (K, 4), dev),
+                D.check(x0, "x0", f64, (B, 3), dev), D.check(end_heading, "end_heading", f64, (B,), dev)]
+        outs = [D.check(states, "states", f64, shape, dev), D.check(n_out, "n_out", i32, (B,), dev),
+                D.check(ok, "ok", i32, (B,), dev), D.check(status, "status", i32, (B,), dev),
+                D.check(iters, "iters", i32, (B,), dev), D.check(bounds, "bounds", f64, (T, D.BOUNDS_COLS), dev)]
+        st = Stats()
+        rc = self._L.pqp_plan_batch_device(self._h, form, int(bounds_mode), int(output_mode), B, T, int(max_n_points),
+                                           *args, float(output_spacing), int(collision_check), int(max_out), *outs,
+                                           torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
+        if rc != OK:
+            raise PqpError(f"pqp_plan_batch_device failed (rc={rc}): {_lib.last_error()}")
+        return dict(states=states, n_out=n_out, ok=ok, status=status, iters=iters, bounds=bounds,
+                    stats=st if stats else None)

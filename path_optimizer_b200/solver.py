@@ -98,6 +98,47 @@ class BatchPathSolver:
             raise PqpError(f"pqp_solve_batch failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, frenet=frenet, status=status, iters=iters, ok=(status == SOLVED), stats=stats)
 
+    def _cuda_device(self):
+        import torch
+        return torch.device("cuda", int(self.device))
+
+    def solve_device(self, n_points, offsets, ref, bounds, x0, end_heading, formulation="KP", max_n_points=0,
+                     min_keep=0, max_keep=0, max_k=None, max_kp=None, want_frenet=True, out=None, stats=False):
+        """The batch as torch CUDA tensors on the solver's device (path_optimizer_b200.device): n_points int32 [B],
+        offsets int32 [B + 1], ref float64 [T, 7], bounds float64 [T, 8], x0 float64 [B, 3], end_heading float64 [B],
+        KPC limits float64 [T].  Every path runs on the kernel class solve() would choose for it, picked on the device
+        (pqp_solve_batch_device_dispatch), with solve()'s results bit for bit.  Runs on torch.cuda.current_stream()
+        without synchronising it (unless `stats`), so that after one warm-up call it can be captured in a CUDA graph.
+        max_n_points / min_keep / max_keep (0 = unknown) only narrow the classes launched; a path outside them reports
+        INVALID_PROBLEM.  `out` may carry the output tensors (states, frenet, status, iters).  Returns them as a dict."""
+        import torch
+        from . import device as D
+        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
+        dev = self._cuda_device()
+        B, T = int(n_points.shape[0]), int(ref.shape[0])
+        out = dict(out or {})
+        f64, i32 = torch.float64, torch.int32
+        states = out.get("states")
+        states = states if states is not None else torch.empty((T, D.STATE_COLS), dtype=f64, device=dev)
+        frenet = out.get("frenet") if want_frenet else None
+        if want_frenet and frenet is None:
+            frenet = torch.empty((T, 3), dtype=f64, device=dev)
+        status = out.get("status") if out.get("status") is not None else torch.empty(B, dtype=i32, device=dev)
+        iters = out.get("iters") if out.get("iters") is not None else torch.empty(B, dtype=i32, device=dev)
+        args = [D.check(n_points, "n_points", i32, (B,), dev), D.check(offsets, "offsets", i32, (B + 1,), dev),
+                D.check(ref, "ref", f64, (T, D.STATE_COLS), dev), D.check(bounds, "bounds", f64, (T, D.BOUNDS_COLS), dev),
+                D.check(x0, "x0", f64, (B, 3), dev), D.check(end_heading, "end_heading", f64, (B,), dev),
+                D.check(max_k, "max_k", f64, (T,), dev), D.check(max_kp, "max_kp", f64, (T,), dev),
+                D.check(states, "states", f64, (T, D.STATE_COLS), dev), D.check(frenet, "frenet", f64, (T, 3), dev),
+                D.check(status, "status", i32, (B,), dev), D.check(iters, "iters", i32, (B,), dev)]
+        st = Stats()
+        rc = self._L.pqp_solve_batch_device_dispatch(self._h, form, B, T, int(max_n_points), int(min_keep), int(max_keep),
+                                                     *args, torch.cuda.current_stream(dev).cuda_stream,
+                                                     C.byref(st) if stats else None)
+        if rc != OK:
+            raise PqpError(f"pqp_solve_batch_device_dispatch failed (rc={rc}): {_lib.last_error()}")
+        return dict(states=states, frenet=frenet, status=status, iters=iters, stats=st if stats else None)
+
 
 class OsqpSolver:
     """Single-path adaptor with the reference's call shape (solver.hpp:31-36)."""
