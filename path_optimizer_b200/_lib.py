@@ -16,7 +16,8 @@ SYMBOLS = ["pqp_params_default", "pqp_params_update_config", "pqp_keep_control_s
            "pqp_solve_batch_device_dispatch", "pqp_class_table"]
 # ... and include/pqp_env.h
 ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "pqp_map_distance", "pqp_spline_fit", "pqp_spline_eval", "pqp_update_bounds_batch",
-               "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device"]
+               "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device",
+               "pqp_set_maps", "pqp_plan_batch_maps", "pqp_plan_batch_device_maps"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -76,6 +77,11 @@ def load():
                                  [C.c_double, C.c_int, C.c_int] + [vp] * 6 + [C.POINTER(Stats)])
     L.pqp_plan_batch_device.argtypes = ([vp] + [C.c_int] * 6 + [vp] * 9 + [C.c_double, C.c_int, C.c_int] + [vp] * 7 +
                                         [C.POINTER(Stats)])
+    L.pqp_set_maps.argtypes = [vp, C.c_int, C.POINTER(DistanceMap)]
+    L.pqp_plan_batch_maps.argtypes = ([vp, C.c_int, C.c_int, C.c_int, C.c_int] + [vp] * 9 +
+                                      [C.c_double, C.c_int, C.c_int] + [vp] * 6 + [C.POINTER(Stats)])
+    L.pqp_plan_batch_device_maps.argtypes = ([vp] + [C.c_int] * 6 + [vp] * 10 + [C.c_double, C.c_int, C.c_int] +
+                                             [vp] * 7 + [C.POINTER(Stats)])
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

@@ -20,16 +20,22 @@
 namespace {
 
 using pqp::CarCircles;
+using pqp::MapTable;
 using pqp::MapView;
 using pqp::SplineView;
 
 struct EnvState {
+    // the map set (pqp_set_maps): every map's cells one after the other, a device table of one descriptor per map and
+    // the device copy of the count; all grow-only, so that a captured chain keeps reading the current set
     float *d_map = nullptr;
     size_t map_cap = 0;
-    MapView mv{};
-    bool has_map = false;
+    MapView *d_maps = nullptr;
+    size_t maps_cap = 0;
+    int32_t *d_nmaps = nullptr;
+    int n_maps = 0;                // 0: no map set
     // per-batch scratch (sized from the handle's capacity at first use)
     int32_t *d_nvalid = nullptr, *d_nkept = nullptr, *d_ok = nullptr, *d_koff = nullptr;
+    int32_t *d_mapidx = nullptr;   // pqp_plan_batch_maps: the uploaded map index
     double *d_spl = nullptr;       // densify workspace: 13 doubles per station
     pqp_state *d_dense = nullptr;  // densify output [batch][max_out] (grow-only)
     size_t dense_cap = 0;
@@ -44,7 +50,8 @@ struct EnvState {
 
 void env_free(void *p) {
     EnvState *e = (EnvState *)p;
-    cudaFree(e->d_map); cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
+    cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx);
+    cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
     cudaFree(e->d_tmp);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
@@ -63,6 +70,9 @@ int env_get(pqp_handle *h, EnvState **out) {
         PQP_CUDA(cudaMalloc(&e->d_nkept, B * sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_ok, B * sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_koff, (B + 1) * sizeof(int32_t)));
+        PQP_CUDA(cudaMalloc(&e->d_mapidx, B * sizeof(int32_t)));
+        PQP_CUDA(cudaMalloc(&e->d_nmaps, sizeof(int32_t)));
+        PQP_CUDA(cudaMemset(e->d_nmaps, 0, sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_spl, T * 13 * sizeof(double)));
         for (auto &ev : e->ev) PQP_CUDA(cudaEventCreate(&ev));
     }
@@ -86,7 +96,7 @@ int grow(T **p, size_t *cap, size_t need_bytes) {
 // ---------------------------------------------------------------------------------------------
 
 struct BoundsArgs {
-    MapView map;
+    MapTable maps;
     double radius;
     double d[4];
     int mode;
@@ -107,6 +117,12 @@ pqp_bounds_kernel(const __grid_constant__ BoundsArgs a) {
     const int i = t >> 2, j = t & 3;
     const int n = a.n_points[b];
     if (i >= n) return;
+    const MapView *mp = pqp::map_of(a.maps, b);
+    if (!mp) {                     // map index outside the set: no usable station, the QP reports PQP_INVALID_PROBLEM
+        if (t == 0) a.n_valid[b] = 0;
+        return;
+    }
+    const MapView map = *mp;
     const int off = a.offsets[b];
     const pqp_state st = a.ref[off + i];
     SplineView xs{0, nullptr, nullptr}, ys{0, nullptr, nullptr};
@@ -116,26 +132,33 @@ pqp_bounds_kernel(const __grid_constant__ BoundsArgs a) {
         ys = SplineView{nk, a.knots + k0, a.yc + 4 * (size_t)k0};
     }
     double ub, lb;
-    const bool blocked = pqp::circle_bounds(a.map, a.radius, a.mode, st, a.d[j], xs, ys, ub, lb);
+    const bool blocked = pqp::circle_bounds(map, a.radius, a.mode, st, a.d[j], xs, ys, ub, lb);
     double *o = &a.out[off + i].c0_ub + 2 * j;
     o[0] = ub;
     o[1] = lb;
     if (blocked) atomicMin(&a.n_valid[b], i);
 }
 
-__global__ void pqp_map_distance_kernel(const __grid_constant__ MapView map, int n, const double *xy, double *out) {
+// The single-stage lookups read map 0 of the set (the entry points check that a set is in place).
+__global__ void pqp_map_distance_kernel(const MapView *maps, int n, const double *xy, double *out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = pqp::map_distance(map, xy[2 * i], xy[2 * i + 1]);
+    if (i >= n) return;
+    const MapView map = maps[0];
+    out[i] = pqp::map_distance(map, xy[2 * i], xy[2 * i + 1]);
 }
 
-__global__ void pqp_check_states_kernel(const __grid_constant__ MapView map, const __grid_constant__ CarCircles car,
-                                        int n, const pqp_state *s, int32_t *ok) {
+__global__ void pqp_check_states_kernel(const MapView *maps, const __grid_constant__ CarCircles car, int n,
+                                        const pqp_state *s, int32_t *ok) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) ok[i] = pqp::state_collision_free(map, car, s[i].x, s[i].y, s[i].z) ? 1 : 0;
+    if (i >= n) return;
+    const MapView map = maps[0];
+    ok[i] = pqp::state_collision_free(map, car, s[i].x, s[i].y, s[i].z) ? 1 : 0;
 }
 
+// The tails look their path's map up once per CTA (thread 0, into shared memory).  Without a collision check the map
+// is not read at all, and no map set is needed.
 struct TailArgs {
-    MapView map;
+    MapTable maps;
     CarCircles car;
     const int32_t *n_points, *offsets;
     const int32_t *status;   // optional: tail only for PQP_SOLVED paths (plan chain)
@@ -148,7 +171,8 @@ struct TailArgs {
 // reference's serial order while every thread checks footprints; the cut is the first failure.
 __global__ void __launch_bounds__(128)
 pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
-    __shared__ int first_fail;
+    __shared__ int first_fail, has_map;
+    __shared__ MapView map_s;
     const int b = blockIdx.x;
     const int n = a.n_points[b];
     pqp_state *p = a.paths + a.offsets[b];
@@ -156,11 +180,21 @@ pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
         if (threadIdx.x == 0) { a.n_kept[b] = 0; a.ok[b] = 0; }
         return;
     }
-    if (threadIdx.x == 0) first_fail = n;
+    if (threadIdx.x == 0) {
+        first_fail = n;
+        const MapView *mp = a.collision_check ? pqp::map_of(a.maps, b) : nullptr;
+        has_map = mp != nullptr;
+        map_s = mp ? *mp : MapView{};
+    }
     __syncthreads();
+    if (a.collision_check && !has_map) {   // map index outside the set
+        if (threadIdx.x == 0) { a.n_kept[b] = 0; a.ok[b] = 0; }
+        return;
+    }
     if (a.collision_check) {
+        const MapView map = map_s;
         for (int i = threadIdx.x; i < n; i += blockDim.x)
-            if (!pqp::state_collision_free(a.map, a.car, p[i].x, p[i].y, p[i].z)) atomicMin(&first_fail, i);
+            if (!pqp::state_collision_free(map, a.car, p[i].x, p[i].y, p[i].z)) atomicMin(&first_fail, i);
     }
     if (threadIdx.x == 0) {
         pqp::accumulate_s(n, p);
@@ -174,7 +208,7 @@ pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
 }
 
 struct DensifyArgs {
-    MapView map;
+    MapTable maps;
     CarCircles car;
     const int32_t *n_points, *offsets, *status;
     const pqp_state *paths;
@@ -189,7 +223,8 @@ struct DensifyArgs {
 // then all threads evaluate / check the samples.
 __global__ void __launch_bounds__(128)
 pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
-    __shared__ int first_fail;
+    __shared__ int first_fail, has_map;
+    __shared__ MapView map_s;
     const int b = blockIdx.x;
     const int n = a.n_points[b];
     const int off = a.offsets[b];
@@ -202,8 +237,18 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
     double *ws = a.ws + 13 * (size_t)off;
     double *t = ws, *xc = ws + n, *yc = ws + 5 * (size_t)n, *scr = ws + 9 * (size_t)n;
     for (int i = threadIdx.x; i < n; i += blockDim.x) t[i] = p[i].s;
-    if (threadIdx.x == 0) first_fail = 0x7fffffff;
+    if (threadIdx.x == 0) {
+        first_fail = 0x7fffffff;
+        const MapView *mp = a.collision_check ? pqp::map_of(a.maps, b) : nullptr;
+        has_map = mp != nullptr;
+        map_s = mp ? *mp : MapView{};
+    }
     __syncthreads();
+    if (a.collision_check && !has_map) {   // map index outside the set
+        if (threadIdx.x == 0) { a.n_out[b] = 0; a.ok[b] = 0; }
+        return;
+    }
+    const MapView map = map_s;
     // threads 0 and 32 fit x(s) and y(s) side by side (diag / rhs scratch: 2n doubles each)
     if (threadIdx.x == 0) pqp::spline_fit(n, t, [&](int i) { return p[i].x; }, xc, scr, scr + n);
     if (threadIdx.x == 32) pqp::spline_fit(n, t, [&](int i) { return p[i].y; }, yc, scr + 2 * (size_t)n, scr + 3 * (size_t)n);
@@ -220,7 +265,7 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
     const long long lim = cnt < (long long)a.max_out + 1 ? cnt : (long long)a.max_out + 1;   // samples that matter
     for (long long i = threadIdx.x; i < lim; i += blockDim.x) {
         const pqp_state st = pqp::densify_sample(xs, ys, pqp::mul((double)i, a.spacing));
-        if (a.collision_check && !pqp::state_collision_free(a.map, a.car, st.x, st.y, st.z)) atomicMin(&first_fail, (int)i);
+        if (a.collision_check && !pqp::state_collision_free(map, a.car, st.x, st.y, st.z)) atomicMin(&first_fail, (int)i);
         if (i < a.max_out) out[i] = st;
     }
     __syncthreads();
@@ -246,12 +291,15 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
 int need_map(pqp_handle *h, EnvState **e) {
     int rc = env_get(h, e);
     if (rc != PQP_OK) return rc;
-    if (!(*e)->has_map) {
-        pqp_set_err("no distance map: call pqp_set_map first");
+    if ((*e)->n_maps < 1) {
+        pqp_set_err("no distance map: call pqp_set_map or pqp_set_maps first");
         return PQP_ERR_ARG;
     }
     return PQP_OK;
 }
+
+// The handle's map set for the kernels; `index` [batch] on the device, or NULL for map 0.
+MapTable map_table(const EnvState *e, const int32_t *index) { return MapTable{e->d_maps, e->d_nmaps, index}; }
 
 // uploads n_points/offsets/ref (+ splines) into the handle's buffers; returns total and max n
 int upload_paths(pqp_handle *h, EnvState *e, int batch, const int32_t *n_points, const pqp_state *ref, int mode,
@@ -320,9 +368,9 @@ PathsView handle_paths(pqp_handle *h, EnvState *e) {
 }
 
 int launch_bounds_kernel(pqp_handle *h, EnvState *e, int mode, int batch, int max_n, const PathsView &p,
-                         pqp_station_bounds *out, cudaStream_t st) {
+                         const int32_t *map_index, pqp_station_bounds *out, cudaStream_t st) {
     BoundsArgs a;
-    a.map = e->mv;
+    a.maps = map_table(e, map_index);
     a.radius = h->params.circle_radius;
     a.d[0] = h->params.d1; a.d[1] = h->params.d2; a.d[2] = h->params.d3; a.d[3] = h->params.d4;
     a.mode = mode;
@@ -347,25 +395,52 @@ int launch_bounds_kernel(pqp_handle *h, EnvState *e, int mode, int batch, int ma
 // ---------------------------------------------------------------------------------------------
 extern "C" {
 
-int pqp_set_map(pqp_handle *h, const pqp_distance_map *map) {
-    if (!h || !map || !map->distance || map->rows < 1 || map->cols < 1 || !(map->resolution > 0.0)) {
-        pqp_set_err("pqp_set_map: bad argument");
+int pqp_set_maps(pqp_handle *h, int n_maps, const pqp_distance_map *maps) {
+    if (!h || n_maps < 1 || !maps) {
+        pqp_set_err("pqp_set_maps: bad argument (needs a handle and n_maps >= 1 descriptors)");
         return PQP_ERR_ARG;
+    }
+    // every descriptor is checked before any device state changes: a bad one leaves the previous set in place
+    for (int m = 0; m < n_maps; ++m) {
+        const pqp_distance_map &d = maps[m];
+        if (!d.distance || d.rows < 1 || d.cols < 1 || !(d.resolution > 0.0)) {
+            pqp_set_err("pqp_set_maps: bad map descriptor (NULL distance, rows or cols < 1, or resolution <= 0)");
+            return PQP_ERR_ARG;
+        }
     }
     EnvState *e;
     int rc = env_get(h, &e);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaSetDevice(h->device));
-    const size_t bytes = (size_t)map->rows * map->cols * sizeof(float);
-    e->has_map = false;
-    rc = grow(&e->d_map, &e->map_cap, bytes);
+    // each map starts on a 256-byte boundary of the one cell buffer
+    constexpr size_t kAlign = 256 / sizeof(float);
+    std::vector<size_t> first((size_t)n_maps);
+    size_t cells = 0;
+    for (int m = 0; m < n_maps; ++m) {
+        first[m] = cells;
+        cells += ((size_t)maps[m].rows * (size_t)maps[m].cols + kAlign - 1) / kAlign * kAlign;
+    }
+    e->n_maps = 0;   // no set until the new one is in place
+    rc = grow(&e->d_map, &e->map_cap, cells * sizeof(float));
     if (rc != PQP_OK) return rc;
-    PQP_CUDA(cudaMemcpyAsync(e->d_map, map->distance, bytes, cudaMemcpyHostToDevice, h->stream));
+    rc = grow(&e->d_maps, &e->maps_cap, (size_t)n_maps * sizeof(MapView));
+    if (rc != PQP_OK) return rc;
+    std::vector<MapView> table((size_t)n_maps);
+    for (int m = 0; m < n_maps; ++m) {
+        const pqp_distance_map &d = maps[m];
+        float *dst = e->d_map + first[m];
+        PQP_CUDA(cudaMemcpyAsync(dst, d.distance, (size_t)d.rows * d.cols * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+        table[m] = pqp::make_map_view(dst, d.rows, d.cols, d.resolution, d.center_x, d.center_y);
+    }
+    const int32_t count = n_maps;
+    PQP_CUDA(cudaMemcpyAsync(e->d_maps, table.data(), table.size() * sizeof(MapView), cudaMemcpyHostToDevice, h->stream));
+    PQP_CUDA(cudaMemcpyAsync(e->d_nmaps, &count, sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
     PQP_CUDA(cudaStreamSynchronize(h->stream));
-    e->mv = pqp::make_map_view(e->d_map, map->rows, map->cols, map->resolution, map->center_x, map->center_y);
-    e->has_map = true;
+    e->n_maps = n_maps;
     return PQP_OK;
 }
+
+int pqp_set_map(pqp_handle *h, const pqp_distance_map *map) { return pqp_set_maps(h, 1, map); }
 
 int pqp_map_distance(pqp_handle *h, int n, const double *xy, double *out) {
     if (!h || n < 0 || (n > 0 && (!xy || !out))) { pqp_set_err("pqp_map_distance: bad argument"); return PQP_ERR_ARG; }
@@ -378,7 +453,7 @@ int pqp_map_distance(pqp_handle *h, int n, const double *xy, double *out) {
     double *d_xy = (double *)e->d_tmp, *d_out = d_xy + 2 * (size_t)n;
     cudaStream_t st = h->stream;
     PQP_CUDA(cudaMemcpyAsync(d_xy, xy, (size_t)n * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
-    pqp_map_distance_kernel<<<(n + 127) / 128, 128, 0, st>>>(e->mv, n, d_xy, d_out);
+    pqp_map_distance_kernel<<<(n + 127) / 128, 128, 0, st>>>(e->d_maps, n, d_xy, d_out);
     PQP_CUDA(cudaGetLastError());
     PQP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, st));
     PQP_CUDA(cudaStreamSynchronize(st));
@@ -447,7 +522,7 @@ int pqp_update_bounds_batch(pqp_handle *h, int mode, int batch, const int32_t *n
     rc = upload_paths(h, e, batch, n_points, ref, mode, n_knots, knots, x_coef, y_coef, &total, &max_n, &h2d, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
-    rc = launch_bounds_kernel(h, e, mode, batch, max_n, handle_paths(h, e), h->d_bounds, st);
+    rc = launch_bounds_kernel(h, e, mode, batch, max_n, handle_paths(h, e), nullptr, h->d_bounds, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[2], st));
     PQP_CUDA(cudaMemcpyAsync(out_bounds, h->d_bounds, (size_t)total * sizeof(pqp_station_bounds), cudaMemcpyDeviceToHost, st));
@@ -526,7 +601,7 @@ int pqp_check_states(pqp_handle *h, int n, const pqp_state *states, int32_t *ok)
     cudaStream_t st = h->stream;
     PQP_CUDA(cudaMemcpyAsync(d_s, states, (size_t)n * sizeof(pqp_state), cudaMemcpyHostToDevice, st));
     const CarCircles car = pqp::make_car_circles(h->params);
-    pqp_check_states_kernel<<<(n + 127) / 128, 128, 0, st>>>(e->mv, car, n, d_s, d_ok);
+    pqp_check_states_kernel<<<(n + 127) / 128, 128, 0, st>>>(e->d_maps, car, n, d_s, d_ok);
     PQP_CUDA(cudaGetLastError());
     PQP_CUDA(cudaMemcpyAsync(ok, d_ok, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     PQP_CUDA(cudaStreamSynchronize(st));
@@ -555,7 +630,7 @@ int pqp_finish_raw_batch(pqp_handle *h, int batch, const int32_t *n_points, pqp_
     PQP_CUDA(cudaMemcpyAsync(h->d_out, h->d_ref, (size_t)total * sizeof(pqp_state), cudaMemcpyDeviceToDevice, st));
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
     TailArgs a;
-    a.map = e->mv; a.car = pqp::make_car_circles(h->params);
+    a.maps = map_table(e, nullptr); a.car = pqp::make_car_circles(h->params);
     a.n_points = h->d_n; a.offsets = h->d_off; a.status = nullptr; a.paths = h->d_out;
     a.collision_check = collision_check ? 1 : 0;
     a.n_kept = e->d_nkept; a.ok = e->d_ok;
@@ -579,10 +654,11 @@ int pqp_finish_raw_batch(pqp_handle *h, int batch, const int32_t *n_points, pqp_
 }
 
 static int launch_densify(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
-                          const int32_t *d_status, const pqp_state *d_paths, double spacing, int collision_check,
-                          int max_out, pqp_state *d_out, int32_t *d_n_out, int32_t *d_ok, cudaStream_t st) {
+                          const int32_t *d_status, const int32_t *d_map_index, const pqp_state *d_paths, double spacing,
+                          int collision_check, int max_out, pqp_state *d_out, int32_t *d_n_out, int32_t *d_ok,
+                          cudaStream_t st) {
     DensifyArgs a;
-    a.map = e->mv; a.car = pqp::make_car_circles(h->params);
+    a.maps = map_table(e, d_map_index); a.car = pqp::make_car_circles(h->params);
     a.n_points = d_n; a.offsets = d_off; a.status = d_status; a.paths = d_paths;
     a.ws = e->d_spl; a.spacing = spacing; a.collision_check = collision_check ? 1 : 0; a.max_out = max_out;
     a.out = d_out; a.n_out = d_n_out; a.ok = d_ok;
@@ -614,8 +690,8 @@ int pqp_densify_batch(pqp_handle *h, int batch, const int32_t *n_points, const p
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
     rc = grow(&e->d_dense, &e->dense_cap, (size_t)batch * (size_t)max_out * sizeof(pqp_state));
     if (rc != PQP_OK) return rc;
-    rc = launch_densify(h, e, batch, h->d_n, h->d_off, nullptr, h->d_ref, output_spacing, collision_check, max_out,
-                        e->d_dense, e->d_nkept, e->d_ok, st);
+    rc = launch_densify(h, e, batch, h->d_n, h->d_off, nullptr, nullptr, h->d_ref, output_spacing, collision_check,
+                        max_out, e->d_dense, e->d_nkept, e->d_ok, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[2], st));
     PQP_CUDA(cudaMemcpyAsync(out_states, e->d_dense, (size_t)batch * max_out * sizeof(pqp_state), cudaMemcpyDeviceToHost, st));
@@ -635,13 +711,14 @@ int pqp_densify_batch(pqp_handle *h, int batch, const int32_t *n_points, const p
 }
 
 // ---- the plan chain: one body on device pointers, two front ends ---------------------------------------------
-// pqp_plan_batch uploads host buffers into the handle's, runs the body and downloads; pqp_plan_batch_device runs the
-// body on the caller's device arrays.
+// pqp_plan_batch_maps uploads host buffers into the handle's, runs the body and downloads; pqp_plan_batch_device_maps
+// runs the body on the caller's device arrays.  pqp_plan_batch and pqp_plan_batch_device are the same with no index.
 struct ChainIO {
     int formulation, bounds_mode, output_mode, batch;
     int max_n;                      // >= every n_points[b]: sizes the bounds grid
     size_t total;
     PathsView paths;
+    const int32_t *map_index;       // [batch] map of every path (bounds and collision check), NULL: map 0
     const double *x0, *end_heading;
     double spacing;
     int collision_check, max_out;
@@ -660,7 +737,7 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     PQP_CUDA(cudaMemsetAsync(c.qp_states, 0, c.total * sizeof(pqp_state), st));   // stations past a cut read as zeros
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[1], st));
     // (1) bounds; n_valid = unblocked prefix of every path
-    int rc = launch_bounds_kernel(h, e, c.bounds_mode, c.batch, c.max_n, c.paths, c.bounds, st);
+    int rc = launch_bounds_kernel(h, e, c.bounds_mode, c.batch, c.max_n, c.paths, c.map_index, c.bounds, st);
     if (rc != PQP_OK) return rc;
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[2], st));
     // (2) QP on the unblocked prefix, every path on the kernel class of its own (length, keep_control_steps), exactly
@@ -693,14 +770,14 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     // (3) tail
     if (c.output_mode == PQP_OUTPUT_RAW) {
         TailArgs a;
-        a.map = e->mv; a.car = pqp::make_car_circles(h->params);
+        a.maps = map_table(e, c.map_index); a.car = pqp::make_car_circles(h->params);
         a.n_points = e->d_nvalid; a.offsets = c.paths.offsets; a.status = c.status; a.paths = c.qp_states;
         a.collision_check = c.collision_check ? 1 : 0;
         a.n_kept = c.out_n; a.ok = c.out_ok;
         pqp_finish_raw_kernel<<<c.batch, 128, 0, st>>>(a);
         PQP_CUDA(cudaGetLastError());
     } else {
-        rc = launch_densify(h, e, c.batch, e->d_nvalid, c.paths.offsets, c.status, c.qp_states, c.spacing,
+        rc = launch_densify(h, e, c.batch, e->d_nvalid, c.paths.offsets, c.status, c.map_index, c.qp_states, c.spacing,
                             c.collision_check, c.max_out, c.dense, c.out_n, c.out_ok, st);
         if (rc != PQP_OK) return rc;
     }
@@ -708,20 +785,21 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     return PQP_OK;
 }
 
-int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, const int32_t *n_points,
-                   const pqp_state *ref, const int32_t *n_knots, const double *knots, const double *x_coef,
-                   const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
-                   int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
-                   int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
+int pqp_plan_batch_maps(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                        const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                        const int32_t *n_knots, const double *knots, const double *x_coef, const double *y_coef,
+                        const double *x0, const double *end_heading, double output_spacing, int collision_check,
+                        int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok, int32_t *status,
+                        int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
     if (!h || batch < 0 || (batch > 0 && (!n_points || !ref || !x0 || !end_heading || !out_states || !out_n || !out_ok)) ||
         (bounds_mode != PQP_BOUNDS_IMPROVED && bounds_mode != PQP_BOUNDS_SIMPLE) ||
         (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
         (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch: bad argument");
+        pqp_set_err("pqp_plan_batch(_maps): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch: unknown formulation");
+        pqp_set_err("pqp_plan_batch(_maps): unknown formulation");
         return PQP_ERR_ARG;
     }
     if (stats) memset(stats, 0, sizeof(*stats));
@@ -740,13 +818,18 @@ int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_m
     PQP_CUDA(cudaMemcpyAsync(h->d_x0, x0, B * 3 * sizeof(double), cudaMemcpyHostToDevice, st));
     PQP_CUDA(cudaMemcpyAsync(h->d_end, end_heading, B * sizeof(double), cudaMemcpyHostToDevice, st));
     h2d += (int64_t)(B * 4 * sizeof(double));
+    if (map_index) {
+        PQP_CUDA(cudaMemcpyAsync(e->d_mapidx, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        h2d += (int64_t)(B * sizeof(int32_t));
+    }
     if (output_mode == PQP_OUTPUT_DENSIFY) {
         rc = grow(&e->d_dense, &e->dense_cap, B * (size_t)max_out * sizeof(pqp_state));
         if (rc != PQP_OK) return rc;
     }
     ChainIO c;
     c.formulation = formulation; c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
-    c.max_n = max_n; c.total = T; c.paths = handle_paths(h, e); c.x0 = h->d_x0; c.end_heading = h->d_end;
+    c.max_n = max_n; c.total = T; c.paths = handle_paths(h, e); c.map_index = map_index ? e->d_mapidx : nullptr;
+    c.x0 = h->d_x0; c.end_heading = h->d_end;
     c.spacing = output_spacing; c.collision_check = collision_check; c.max_out = max_out;
     c.qp_states = h->d_out; c.dense = e->d_dense; c.out_n = e->d_nkept; c.out_ok = e->d_ok;
     c.status = h->d_status; c.iters = h->d_iters; c.bounds = h->d_bounds;
@@ -796,13 +879,24 @@ int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_m
     return PQP_OK;
 }
 
-int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, int total_points,
-                          int max_n_points, const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
-                          const int32_t *d_knot_offsets, const double *d_knots, const double *d_x_coef,
-                          const double *d_y_coef, const double *d_x0, const double *d_end_heading, double output_spacing,
-                          int collision_check, int max_out, pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok,
-                          int32_t *d_status, int32_t *d_iters, pqp_station_bounds *d_out_bounds, void *stream,
-                          pqp_stats *stats) {
+int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, const int32_t *n_points,
+                   const pqp_state *ref, const int32_t *n_knots, const double *knots, const double *x_coef,
+                   const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
+                   int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
+                   int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
+    return pqp_plan_batch_maps(h, formulation, bounds_mode, output_mode, batch, n_points, ref, nullptr, n_knots, knots,
+                               x_coef, y_coef, x0, end_heading, output_spacing, collision_check, max_out, out_states,
+                               out_n, out_ok, status, iters, out_bounds, stats);
+}
+
+int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                               int total_points, int max_n_points, const int32_t *d_n_points, const int32_t *d_offsets,
+                               const pqp_state *d_ref, const int32_t *d_map_index, const int32_t *d_knot_offsets,
+                               const double *d_knots, const double *d_x_coef, const double *d_y_coef,
+                               const double *d_x0, const double *d_end_heading, double output_spacing,
+                               int collision_check, int max_out, pqp_state *d_out_states, int32_t *d_out_n,
+                               int32_t *d_out_ok, int32_t *d_status, int32_t *d_iters,
+                               pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
     if (!h || batch < 0 || total_points < 0 ||
         (batch > 0 && (!d_n_points || !d_offsets || !d_ref || !d_x0 || !d_end_heading || !d_out_states || !d_out_n ||
                        !d_out_ok || !d_status)) ||
@@ -810,11 +904,11 @@ int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int o
         (bounds_mode == PQP_BOUNDS_IMPROVED && batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef)) ||
         (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
         (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch_device: bad argument");
+        pqp_set_err("pqp_plan_batch_device(_maps): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch_device: unknown formulation");
+        pqp_set_err("pqp_plan_batch_device(_maps): unknown formulation");
         return PQP_ERR_ARG;
     }
     if (stats) memset(stats, 0, sizeof(*stats));
@@ -833,6 +927,7 @@ int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int o
     c.max_n = max_n_points > 0 ? max_n_points : h->cls_ncols[formulation] - 2;
     c.total = (size_t)total_points;
     c.paths = PathsView{d_n_points, d_offsets, d_ref, d_knot_offsets, d_knots, d_x_coef, d_y_coef};
+    c.map_index = d_map_index;
     c.x0 = d_x0; c.end_heading = d_end_heading;
     c.spacing = output_spacing; c.collision_check = collision_check; c.max_out = max_out;
     c.qp_states = output_mode == PQP_OUTPUT_RAW ? d_out_states : h->d_out;
@@ -852,6 +947,19 @@ int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int o
         stats->kernel_launches = 2 + qp_launches;
     }
     return PQP_OK;
+}
+
+int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, int total_points,
+                          int max_n_points, const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                          const int32_t *d_knot_offsets, const double *d_knots, const double *d_x_coef,
+                          const double *d_y_coef, const double *d_x0, const double *d_end_heading, double output_spacing,
+                          int collision_check, int max_out, pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok,
+                          int32_t *d_status, int32_t *d_iters, pqp_station_bounds *d_out_bounds, void *stream,
+                          pqp_stats *stats) {
+    return pqp_plan_batch_device_maps(h, formulation, bounds_mode, output_mode, batch, total_points, max_n_points,
+                                      d_n_points, d_offsets, d_ref, nullptr, d_knot_offsets, d_knots, d_x_coef,
+                                      d_y_coef, d_x0, d_end_heading, output_spacing, collision_check, max_out,
+                                      d_out_states, d_out_n, d_out_ok, d_status, d_iters, d_out_bounds, stream, stats);
 }
 
 }  // extern "C"

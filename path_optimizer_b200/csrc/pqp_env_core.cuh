@@ -74,6 +74,22 @@ PQP_HD MapView make_map_view(const float *d, int rows, int cols, double res, dou
     return m;
 }
 
+// The map set of a handle (pqp_set_maps) as the kernels see it: a device table with one descriptor per map, the number
+// of maps, and an optional per-path index into the table (NULL: map 0 for every path).  The count is read from memory
+// rather than passed by value, so that a captured launch follows a later upload of a set of another size.
+struct MapTable {
+    const MapView *maps;
+    const int32_t *n_maps;
+    const int32_t *index;
+};
+
+// Descriptor of path b's map, or NULL when its index lies outside [0, n_maps): the index is checked before the table
+// is read.
+PQP_HD const MapView *map_of(const MapTable &t, int b) {
+    const int m = t.index ? t.index[b] : 0;
+    return (m >= 0 && m < *t.n_maps) ? t.maps + m : nullptr;
+}
+
 // grid_map isInside: 0 <= -((p - c) - len/2) < len on both axes
 PQP_HD bool map_inside(const MapView &m, double x, double y) {
     const double tx = -add(x - m.cx, -mul(0.5, m.lx));

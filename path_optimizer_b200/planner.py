@@ -79,6 +79,20 @@ class PathPlanner(BatchPathSolver):
         if rc != OK:
             raise PqpError(f"pqp_set_map failed (rc={rc}): {_lib.last_error()}")
 
+    def set_maps(self, maps):
+        """Replace the map set with several maps (pqp_set_maps), each a dict in the form set_map takes; plan() and
+        plan_device() pick a path's map with `map_index`.  The single-stage calls and plan() without an index use
+        map 0."""
+        maps = list(maps)
+        dists = [np.ascontiguousarray(m["distance"], dtype=np.float32) for m in maps]
+        dms = (DistanceMap * max(len(maps), 1))()
+        for i, (m, d) in enumerate(zip(maps, dists)):
+            dms[i] = DistanceMap(ptr(d), d.shape[0], d.shape[1], float(m["resolution"]), float(m["center_x"]),
+                                 float(m["center_y"]))
+        rc = self._L.pqp_set_maps(self._h, len(maps), dms)
+        if rc != OK:
+            raise PqpError(f"pqp_set_maps failed (rc={rc}): {_lib.last_error()}")
+
     def map_distance(self, xy):
         xy = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)
         out = np.zeros(len(xy))
@@ -145,9 +159,11 @@ class PathPlanner(BatchPathSolver):
         return dict(states=out, n_out=n_out, ok=ok, stats=stats)
 
     def plan(self, batch, formulation="KP", bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW,
-             output_spacing=0.3, collision_check=True, max_out=512, want_bounds=False, out=None):
+             output_spacing=0.3, collision_check=True, max_out=512, want_bounds=False, out=None, map_index=None):
         """PathOptimizer::solveWithoutSmoothing for every path of the batch (bounds -> QP -> tail).
-        `out` may carry a preallocated (e.g. pinned) `states` array of the output shape."""
+        `out` may carry a preallocated (e.g. pinned) `states` array of the output shape.  `map_index`: int32 [B], the
+        map of the set (set_maps) every path is planned on (pqp_plan_batch_maps); None: map 0 (pqp_plan_batch).  A path
+        whose index is outside the set reports status -100 (invalid problem), 0 iterations, n_out = 0 and ok = 0."""
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
         B = len(n_points)
@@ -167,25 +183,35 @@ class PathPlanner(BatchPathSolver):
         iters = np.zeros(B, dtype=np.int32)
         bounds = np.zeros(len(ref), dtype=BOUNDS_DTYPE) if want_bounds else None
         stats = Stats()
-        rc = self._L.pqp_plan_batch(self._h, form, int(bounds_mode), int(output_mode), B, ptr(n_points), ptr(ref),
-                                    ptr(nk), ptr(kn), ptr(xc), ptr(yc), ptr(x0), ptr(end_heading),
-                                    float(output_spacing), int(collision_check), int(max_out), ptr(states),
-                                    ptr(n_out), ptr(ok), ptr(status), ptr(iters), ptr(bounds), C.byref(stats))
+        head = (self._h, form, int(bounds_mode), int(output_mode), B, ptr(n_points), ptr(ref))
+        tail = (ptr(nk), ptr(kn), ptr(xc), ptr(yc), ptr(x0), ptr(end_heading), float(output_spacing),
+                int(collision_check), int(max_out), ptr(states), ptr(n_out), ptr(ok), ptr(status), ptr(iters),
+                ptr(bounds), C.byref(stats))
+        if map_index is None:
+            name, rc = "pqp_plan_batch", self._L.pqp_plan_batch(*head, *tail)
+        else:
+            mi = np.asarray(map_index)
+            if mi.shape != (B,) or mi.dtype.kind not in "iu":
+                raise ValueError(f"map_index: expected an integer array of shape ({B},), got {mi.dtype} {mi.shape}")
+            mi = np.ascontiguousarray(mi, dtype=np.int32)
+            name, rc = "pqp_plan_batch_maps", self._L.pqp_plan_batch_maps(*head, ptr(mi), *tail)
         if rc != OK:
-            raise PqpError(f"pqp_plan_batch failed (rc={rc}): {_lib.last_error()}")
+            raise PqpError(f"{name} failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, n_out=n_out, ok=ok, status=status, iters=iters, bounds=bounds,
                     solved=(status == SOLVED), stats=stats)
 
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
-                    collision_check=True, max_out=512, want_bounds=False, out=None, stats=False):
+                    collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None):
         """plan() on torch CUDA tensors of the planner's device (path_optimizer_b200.device): n_points int32 [B],
         offsets int32 [B + 1], ref float64 [T, 7], x0 float64 [B, 3], end_heading float64 [B]; `splines` (IMPROVED)
         a dict of knot_offsets int32 [B + 1], knots [K], x_coef / y_coef [K, 4] (device.splines_to_device).  The whole
         chain runs on the device (pqp_plan_batch_device) on torch.cuda.current_stream() with plan()'s results bit for
         bit and no host synchronisation (unless `stats`): after one warm-up call it can be captured in a CUDA graph.
         max_n_points >= every n_points (0: the longest path any kernel class takes).  `out` may carry the output
-        tensors (states: [T, 7] RAW or [B, max_out, 7] DENSIFY; n_out, ok, status, iters; bounds [T, 8])."""
+        tensors (states: [T, 7] RAW or [B, max_out, 7] DENSIFY; n_out, ok, status, iters; bounds [T, 8]).
+        `map_index`: int32 [B] on the device, the map of the set every path is planned on (pqp_plan_batch_device_maps,
+        as plan(map_index=...)); None: map 0.  A graph replay reads the index from the captured tensor."""
         import torch
         from . import device as D
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
@@ -212,10 +238,16 @@ class PathPlanner(BatchPathSolver):
                 D.check(ok, "ok", i32, (B,), dev), D.check(status, "status", i32, (B,), dev),
                 D.check(iters, "iters", i32, (B,), dev), D.check(bounds, "bounds", f64, (T, D.BOUNDS_COLS), dev)]
         st = Stats()
-        rc = self._L.pqp_plan_batch_device(self._h, form, int(bounds_mode), int(output_mode), B, T, int(max_n_points),
-                                           *args, float(output_spacing), int(collision_check), int(max_out), *outs,
-                                           torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
+        head = (self._h, form, int(bounds_mode), int(output_mode), B, T, int(max_n_points))
+        tail = (float(output_spacing), int(collision_check), int(max_out), *outs,
+                torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
+        if map_index is None:
+            name, rc = "pqp_plan_batch_device", self._L.pqp_plan_batch_device(*head, *args, *tail)
+        else:
+            mi = D.check(map_index, "map_index", i32, (B,), dev)
+            name, rc = "pqp_plan_batch_device_maps", self._L.pqp_plan_batch_device_maps(*head, *args[:3], mi, *args[3:],
+                                                                                        *tail)
         if rc != OK:
-            raise PqpError(f"pqp_plan_batch_device failed (rc={rc}): {_lib.last_error()}")
+            raise PqpError(f"{name} failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, n_out=n_out, ok=ok, status=status, iters=iters, bounds=bounds,
                     stats=st if stats else None)

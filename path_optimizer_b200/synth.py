@@ -261,3 +261,46 @@ def infeasible_corridors(batch, n=60, seed=BASE_SEED, first_path=0, config=6):
             bb["c0_lb"][10:], bb["c0_ub"][10:] = 2.0, 2.5
             bb["c2_lb"][10:], bb["c2_ub"][10:] = -2.5, -2.0
     return b
+
+
+# ---------------------------------------------------------------------------------------------
+# Many scenes in one batch (pqp_set_maps + a map index per path)
+# ---------------------------------------------------------------------------------------------
+
+def scene_map(k, seed=BASE_SEED):
+    """Scene k of a many-scene batch: disc_field_map with its own seed.  Every fourth scene (k % 4 == 1) has a 0.25 m
+    resolution and a centre away from the origin, so that a set mixes map geometries."""
+    if k % 4 == 1:
+        return disc_field_map(resolution=0.25, seed=seed + k, center=(35.0 + 10.0 * (k % 7), -20.0 + 3.0 * (k % 5)))
+    return disc_field_map(seed=seed + k)
+
+
+def multi_map_batch(n_maps, n_candidates, n=200, seed=BASE_SEED, first_maps=(), order="grouped", mapper=map, **line_kw):
+    """A batch planned over several maps: `first_maps` (e.g. the config-1 fixture map) followed by scene_map(k) for the
+    remaining scenes up to `n_maps`, and `n_candidates` reference lines of `n` stations per map, placed in that map's
+    frame (map_reference_paths shifted to the map's centre, starting 5 m inside its -x edge or at x = -100 m from the
+    centre, whichever is further in).  `order`: "grouped" (the paths of map 0, then map 1, ...) or "interleaved" (one
+    path of every map in turn).  `mapper` builds the generated maps (e.g. a process pool's map).
+    Returns (maps, batch, map_index int32 [n_maps * n_candidates])."""
+    first_maps = list(first_maps)
+    maps = first_maps + list(mapper(scene_map, range(len(first_maps), n_maps), [seed] * (n_maps - len(first_maps))))
+    parts = []
+    for m, mp in enumerate(maps):
+        lx = mp["rows"] * mp["resolution"]
+        x_lo = max(-lx / 2 + 5.0, -100.0)
+        x_hi = max(x_lo, min(40.0, lx / 2 - 5.0 - 0.3 * n))
+        kw = dict(x_range=(mp["center_x"] + x_lo, mp["center_x"] + x_hi), y_range=(-0.5, 0.5))
+        kw.update(line_kw)
+        kw["y_range"] = (mp["center_y"] + kw["y_range"][0], mp["center_y"] + kw["y_range"][1])
+        parts.append(map_reference_paths(n_candidates, n, seed=seed, first_path=m * n_candidates, **kw))
+    b = dict(n_points=np.concatenate([p["n_points"] for p in parts]), ref=np.concatenate([p["ref"] for p in parts]),
+             bounds=np.concatenate([p["bounds"] for p in parts]), x0=np.concatenate([p["x0"] for p in parts]),
+             end_heading=np.concatenate([p["end_heading"] for p in parts]))
+    b["offsets"] = np.concatenate([[0], np.cumsum(b["n_points"])]).astype(np.int32)
+    map_index = np.repeat(np.arange(n_maps, dtype=np.int32), n_candidates)
+    if order == "interleaved":
+        perm = np.arange(n_maps * n_candidates).reshape(n_maps, n_candidates).T.reshape(-1)
+        b, map_index = take_paths(b, perm), map_index[perm]
+    elif order != "grouped":
+        raise ValueError(f"order: 'grouped' or 'interleaved', got {order!r}")
+    return maps, b, np.ascontiguousarray(map_index, dtype=np.int32)
