@@ -187,8 +187,23 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device,
 void pqp_destroy(pqp_handle *h);
 
 /* Replace the parameter snapshot of an existing handle (the reference re-reads FLAGS_* on
- * every solve, e.g. solver_kp_as_input.cpp:48-51). */
+ * every solve, e.g. solver_kp_as_input.cpp:48-51): pqp_set_param_sets(h, 1, params). */
 int pqp_set_params(pqp_handle *h, const pqp_params *params);
+
+/* Most parameter sets one handle holds. */
+#define PQP_MAX_PARAM_SETS 64
+
+/* Replace the handle's parameter sets with `n_sets` (1..PQP_MAX_PARAM_SETS) snapshots, so that one call can batch paths
+ * of several vehicles, weight sweeps or solver tolerances (pqp_solve_batch_sets, pqp_solve_batch_device_dispatch_sets,
+ * pqp_plan_batch_sets, pqp_plan_batch_device_sets: one set index per path).  Every set is given already run through
+ * pqp_params_update_config, as for pqp_set_params.  Every argument is checked before anything changes: a bad one returns
+ * PQP_ERR_ARG and leaves the previous sets in place.  Synchronous; no caller pointer is kept.  The params given to
+ * pqp_create are set 0; the entries without a set index, and the single-stage entries of pqp_env.h, read set 0.
+ * Every stage takes the sets by value at launch: a CUDA graph captured before this call keeps, at every stage, the sets
+ * it was captured with; capture again to follow the new ones.
+ * Replaces: the FLAGS_* globals the reference reads at call time (solver_kp_as_input.cpp:48-51, 111-127, 155-158;
+ * reference_path_impl.cpp:203-235; updateConfig() from the PathOptimizer constructor), one value set per path. */
+int pqp_set_param_sets(pqp_handle *h, int n_sets, const pqp_params *sets);
 
 /* Solve `batch` independent path QPs.  HOST buffers; H2D / D2H copies happen inside.
  *
@@ -302,6 +317,52 @@ int pqp_solve_batch_device_dispatch(pqp_handle *h, int formulation, int batch, i
                                     int32_t *d_iters,
                                     void *stream,
                                     pqp_stats *stats);
+
+/* pqp_solve_batch and pqp_solve_batch_device_dispatch over the handle's parameter sets (pqp_set_param_sets): the same
+ * arguments plus one set index per path, on the host (`param_index`) or on the device (`d_param_index`), both int32
+ * [batch].  Path b is solved with set param_index[b]: its results equal, bit for bit, those of a handle whose only set
+ * is that one.  A NULL index means set 0 for every path: pqp_solve_batch and pqp_solve_batch_device_dispatch are these
+ * entries with a NULL index.  An index outside [0, n_sets), or for the device entry at or past `n_param_sets`, makes only
+ * that path report PQP_INVALID_PROBLEM (0 iterations, NaN states); the index is checked before the sets are read, and
+ * no other path's results change.
+ *   n_param_sets   device entry: an upper bound on the indices used (0: the handle's set count).  Like max_n_points it
+ *                  bounds what is launched: one grid per (set, kernel class) pair the bounds reach.
+ * The host entry plans one launch segment per (set, class), longest path first inside a segment (pqp_set_order_hint and
+ * the input-derived order still apply inside a segment).  The device entry keeps every promise of
+ * pqp_solve_batch_device_dispatch (asynchronous, no allocation after a warm-up call with the same or a larger
+ * n_param_sets, capturable); its sort needs device scratch that grows with n_param_sets.  With PQP_GENERIC_K /
+ * PQP_GENERIC_KPC set, a non-NULL index returns PQP_ERR_UNSUPPORTED.
+ * Replaces: OsqpSolver::solve (solver.cpp:46-77) once per path, with that path's FLAGS_*. */
+int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch,
+                         const int32_t *n_points,
+                         const pqp_state *ref,
+                         const pqp_station_bounds *bounds,
+                         const double *x0,
+                         const double *end_heading,
+                         const double *max_k,
+                         const double *max_kp,
+                         const int32_t *param_index,
+                         pqp_state *out_states,
+                         double *out_frenet,
+                         int32_t *status,
+                         int32_t *iters,
+                         pqp_stats *stats);
+int pqp_solve_batch_device_dispatch_sets(pqp_handle *h, int formulation, int batch, int total_points,
+                                         int max_n_points, int min_keep, int max_keep, int n_param_sets,
+                                         const int32_t *d_n_points, const int32_t *d_offsets,
+                                         const pqp_state *d_ref,
+                                         const pqp_station_bounds *d_bounds,
+                                         const double *d_x0,
+                                         const double *d_end_heading,
+                                         const double *d_max_k,
+                                         const double *d_max_kp,
+                                         const int32_t *d_param_index,
+                                         pqp_state *d_out_states,
+                                         double *d_out_frenet,
+                                         int32_t *d_status,
+                                         int32_t *d_iters,
+                                         void *stream,
+                                         pqp_stats *stats);
 
 /* Last error text for this thread (CUDA error strings etc.); never NULL. */
 /* Launch-order hint for the next solves of a batch of `batch` paths: expected ADMM iterations per path, e.g. the

@@ -224,6 +224,45 @@ int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, 
                                int32_t *d_status, int32_t *d_iters,
                                pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats);
 
+/* pqp_plan_batch_maps and pqp_plan_batch_device_maps over the handle's parameter sets (pqp_set_param_sets) as well: the
+ * same arguments plus one set index per path (`param_index` on the host, `d_param_index` on the device, int32 [batch])
+ * and, for the device entry, `n_param_sets`, an upper bound on the indices used (0: the handle's set count).
+ *   Path b runs every stage with set param_index[b]: circle radius and d1..d4 of its bounds, the footprint of its
+ *   collision check, the "KPC" limits (mu, curvature rate) and everything the QP reads.  Its results -- status,
+ *   iterations, states, bounds, out_n and ok -- equal, bit for bit, those pqp_plan_batch_maps gives it on a handle whose
+ *   only set is that one.  A NULL index means set 0: the _maps entries are these with a NULL index.
+ *   An index outside [0, n_sets), or for the device entry at or past n_param_sets, makes that path report
+ *   PQP_INVALID_PROBLEM with 0 iterations, out_n = 0 and ok = 0; no other path's results change.  The index is checked
+ *   before the sets are read.
+ * The QP step launches one grid per (set, kernel class) pair (pqp_solve_batch_sets,
+ * pqp_solve_batch_device_dispatch_sets).  The device entry keeps every promise of pqp_plan_batch_device_maps; a CUDA
+ * graph replays with the sets it was captured with, at every stage (the map rule differs: the chain reads the map
+ * descriptors from device memory, so a replay follows a later pqp_set_maps).
+ * Replaces: PathOptimizer::solveWithoutSmoothing (path_optimizer.cpp:87-117) once per path, with that path's FLAGS_*
+ * (and the PathOptimizer of its own scene). */
+int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                        const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                        const int32_t *param_index,
+                        const int32_t *n_knots, const double *knots,
+                        const double *x_coef, const double *y_coef,
+                        const double *x0, const double *end_heading,
+                        double output_spacing, int collision_check, int max_out,
+                        pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
+                        int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds,
+                        pqp_stats *stats);
+int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode,
+                               int batch, int total_points, int max_n_points, int n_param_sets,
+                               const int32_t *d_n_points, const int32_t *d_offsets,
+                               const pqp_state *d_ref, const int32_t *d_map_index,
+                               const int32_t *d_param_index,
+                               const int32_t *d_knot_offsets, const double *d_knots,
+                               const double *d_x_coef, const double *d_y_coef,
+                               const double *d_x0, const double *d_end_heading,
+                               double output_spacing, int collision_check, int max_out,
+                               pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok,
+                               int32_t *d_status, int32_t *d_iters,
+                               pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats);
+
 #ifdef __cplusplus
 } /* extern "C" */
 #endif

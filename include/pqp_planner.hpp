@@ -83,6 +83,20 @@ class PathOptimizerGpu {
         return p;
     }
 
+    // Several parameter sets as well (pqp_set_param_sets): param_sets[k] is set k of the batched solveWithoutSmoothing's
+    // param_index; param_sets[0] is what every call without an index uses.
+    static std::unique_ptr<PathOptimizerGpu> create(const std::vector<DistanceMap> &maps,
+                                                    const std::vector<pqp_params> &param_sets, int max_batch,
+                                                    int max_total_points, int device = 0) {
+        if (param_sets.empty()) return nullptr;
+        std::unique_ptr<PathOptimizerGpu> p = create(maps, max_batch, max_total_points, &param_sets[0], device);
+        if (p && pqp_set_param_sets(p->handle_.get(), (int)param_sets.size(), param_sets.data()) != PQP_OK) {
+            std::fprintf(stderr, "pqp_set_param_sets failed: %s\n", pqp_last_error());
+            return nullptr;
+        }
+        return p;
+    }
+
     double getObstacleDistance(double x, double y) const {
         const double xy[2] = {x, y};
         double d = 0;
@@ -124,7 +138,7 @@ class PathOptimizerGpu {
                                std::vector<std::vector<State>> *final_paths, std::vector<char> *ok,
                                const std::vector<Spline> *x_s = nullptr, const std::vector<Spline> *y_s = nullptr,
                                std::vector<int32_t> *status = nullptr) {
-        return plan(references, vehicle, nullptr, final_paths, ok, x_s, y_s, status);
+        return plan(references, vehicle, nullptr, nullptr, final_paths, ok, x_s, y_s, status);
     }
 
     // The same with map_index[b] naming the map (of those the optimizer was created with) reference b is planned on.
@@ -134,7 +148,21 @@ class PathOptimizerGpu {
                                std::vector<char> *ok, const std::vector<Spline> *x_s = nullptr,
                                const std::vector<Spline> *y_s = nullptr, std::vector<int32_t> *status = nullptr) {
         if (map_index.size() != references.size()) return false;
-        return plan(references, vehicle, map_index.data(), final_paths, ok, x_s, y_s, status);
+        return plan(references, vehicle, map_index.data(), nullptr, final_paths, ok, x_s, y_s, status);
+    }
+
+    // The same with param_index[b] naming the parameter set reference b is planned with as well: PathOptimizer::
+    // solveWithoutSmoothing once per reference with that reference's FLAGS_*.  An empty map_index means map 0 for every
+    // reference.  A reference whose set index names no set gets ok = 0, an empty path and status PQP_INVALID_PROBLEM.
+    bool solveWithoutSmoothing(const std::vector<std::vector<State>> &references, const std::vector<VehicleStateView> &vehicle,
+                               const std::vector<int32_t> &map_index, const std::vector<int32_t> &param_index,
+                               std::vector<std::vector<State>> *final_paths, std::vector<char> *ok,
+                               const std::vector<Spline> *x_s = nullptr, const std::vector<Spline> *y_s = nullptr,
+                               std::vector<int32_t> *status = nullptr) {
+        if ((!map_index.empty() && map_index.size() != references.size()) || param_index.size() != references.size())
+            return false;
+        return plan(references, vehicle, map_index.empty() ? nullptr : map_index.data(), param_index.data(), final_paths,
+                    ok, x_s, y_s, status);
     }
 
     // The reference's single-path signature (path_optimizer.cpp:87-88).
@@ -151,9 +179,11 @@ class PathOptimizerGpu {
     pqp_handle *handle() const { return handle_.get(); }
 
  private:
-    // Batched solveWithoutSmoothing (pqp_plan_batch_maps; map_index NULL: map 0 for every reference).
+    // Batched solveWithoutSmoothing (pqp_plan_batch_sets; map_index NULL: map 0, param_index NULL: set 0 for every
+    // reference).
     bool plan(const std::vector<std::vector<State>> &references, const std::vector<VehicleStateView> &vehicle,
-              const int32_t *map_index, std::vector<std::vector<State>> *final_paths, std::vector<char> *ok,
+              const int32_t *map_index, const int32_t *param_index, std::vector<std::vector<State>> *final_paths,
+              std::vector<char> *ok,
               const std::vector<Spline> *x_s, const std::vector<Spline> *y_s, std::vector<int32_t> *status) {
         const int B = (int)references.size();
         Packed in;
@@ -168,14 +198,14 @@ class PathOptimizerGpu {
         const bool raw = enable_raw_output;
         std::vector<State> out(raw ? in.ref.size() : (size_t)B * max_output_states);
         std::vector<int32_t> n_out(B), okv(B), st(B);
-        const int rc = pqp_plan_batch_maps(handle_.get(), PQP_FORM_KP, in.mode, raw ? PQP_OUTPUT_RAW : PQP_OUTPUT_DENSIFY,
+        const int rc = pqp_plan_batch_sets(handle_.get(), PQP_FORM_KP, in.mode, raw ? PQP_OUTPUT_RAW : PQP_OUTPUT_DENSIFY,
                                            B, in.n.data(), reinterpret_cast<const pqp_state *>(in.ref.data()), map_index,
-                                           in.nk_ptr(), in.knots_ptr(), in.xc_ptr(), in.yc_ptr(), x0.data(), endh.data(),
-                                           output_spacing, enable_collision_check ? 1 : 0, max_output_states,
+                                           param_index, in.nk_ptr(), in.knots_ptr(), in.xc_ptr(), in.yc_ptr(), x0.data(),
+                                           endh.data(), output_spacing, enable_collision_check ? 1 : 0, max_output_states,
                                            reinterpret_cast<pqp_state *>(out.data()), n_out.data(), okv.data(), st.data(),
                                            nullptr, nullptr, nullptr);
         if (rc != PQP_OK) {
-            std::fprintf(stderr, "pqp_plan_batch_maps failed: %s\n", pqp_last_error());
+            std::fprintf(stderr, "pqp_plan_batch_sets failed: %s\n", pqp_last_error());
             return false;
         }
         final_paths->assign(B, {});

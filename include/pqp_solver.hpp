@@ -113,10 +113,41 @@ class BatchPathSolver {
         return s;
     }
 
+    // Several parameter sets on one handle (pqp_set_param_sets): param_sets[k] is set k of solve()'s param_index,
+    // param_sets[0] the set of a solve without one.
+    static std::unique_ptr<BatchPathSolver> create(const std::string &type, int max_batch, int max_total_points,
+                                                   const std::vector<pqp_params> &param_sets, int device = 0) {
+        if (param_sets.empty()) return nullptr;
+        std::unique_ptr<BatchPathSolver> s = create(type, max_batch, max_total_points, &param_sets[0], device);
+        if (s && pqp_set_param_sets(s->handle_.get(), (int)param_sets.size(), param_sets.data()) != PQP_OK) {
+            std::fprintf(stderr, "pqp_set_param_sets failed: %s\n", pqp_last_error());
+            return nullptr;
+        }
+        return s;
+    }
+
     // n_points[b] stations per path; reference_states / bounds concatenated; vehicle[b] per path.
     bool solve(const std::vector<int32_t> &n_points, const std::vector<State> &reference_states,
                const std::vector<CoveringCircleBounds> &bounds, const std::vector<VehicleStateView> &vehicle,
                Result *out) {
+        return solve(n_points, reference_states, bounds, vehicle, nullptr, out);
+    }
+
+    // The same with param_index[b] naming the parameter set path b is solved with (pqp_solve_batch_sets): OsqpSolver::solve
+    // once per path with that path's FLAGS_*.  A path whose index names no set reports PQP_INVALID_PROBLEM.
+    bool solve(const std::vector<int32_t> &n_points, const std::vector<State> &reference_states,
+               const std::vector<CoveringCircleBounds> &bounds, const std::vector<VehicleStateView> &vehicle,
+               const std::vector<int32_t> &param_index, Result *out) {
+        if (param_index.size() != n_points.size()) return false;
+        return solve(n_points, reference_states, bounds, vehicle, param_index.data(), out);
+    }
+
+    pqp_handle *handle() const { return handle_.get(); }
+
+ private:
+    bool solve(const std::vector<int32_t> &n_points, const std::vector<State> &reference_states,
+               const std::vector<CoveringCircleBounds> &bounds, const std::vector<VehicleStateView> &vehicle,
+               const int32_t *param_index, Result *out) {
         const int batch = (int)n_points.size();
         size_t total = 0;
         for (int n : n_points) total += (size_t)n;
@@ -132,18 +163,16 @@ class BatchPathSolver {
         out->frenet.assign(3 * total, 0.0);
         out->status.assign(batch, PQP_UNSOLVED);
         out->iters.assign(batch, 0);
-        out->rc = pqp_solve_batch(handle_.get(), form_, batch, n_points.data(),
-                                  reinterpret_cast<const pqp_state *>(reference_states.data()),
-                                  reinterpret_cast<const pqp_station_bounds *>(bounds.data()), x0.data(),
-                                  endh.data(), nullptr, nullptr, reinterpret_cast<pqp_state *>(out->states.data()),
-                                  out->frenet.data(), out->status.data(), out->iters.data(), &out->stats);
-        if (out->rc != PQP_OK) std::fprintf(stderr, "pqp_solve_batch failed: %s\n", pqp_last_error());
+        out->rc = pqp_solve_batch_sets(handle_.get(), form_, batch, n_points.data(),
+                                       reinterpret_cast<const pqp_state *>(reference_states.data()),
+                                       reinterpret_cast<const pqp_station_bounds *>(bounds.data()), x0.data(),
+                                       endh.data(), nullptr, nullptr, param_index,
+                                       reinterpret_cast<pqp_state *>(out->states.data()), out->frenet.data(),
+                                       out->status.data(), out->iters.data(), &out->stats);
+        if (out->rc != PQP_OK) std::fprintf(stderr, "pqp_solve_batch_sets failed: %s\n", pqp_last_error());
         return out->rc == PQP_OK;
     }
 
-    pqp_handle *handle() const { return handle_.get(); }
-
- private:
     BatchPathSolver() = default;
     Handle handle_;
     int form_ = PQP_FORM_KP;

@@ -210,31 +210,68 @@ bool auto_order_enabled() {
 }
 
 extern "C" {
-static int launch_variant(pqp_handle *h, int v, const pqp::BatchView &bv, int count, const int32_t *d_order,
-                          size_t smem_bytes, cudaStream_t st);
+static int launch_variant(pqp_handle *h, int v, const pqp::DevParams *prm, const pqp::BatchView &bv, int count,
+                          const int32_t *d_order, size_t smem_bytes, cudaStream_t st);
 }
 
-// One launch per class with count_v[v] > 0: count_v[v] CTAs over the order entries d_order + start_v[v], with smem_v[v]
-// bytes.  A mixed batch has several: they go out on the handle's class lanes (forked from and joined back into `st`),
-// the class of the longest paths first, so that the CTAs of the next class fill the SMs the tail of the previous one
-// leaves idle instead of waiting for its last path.
-static int launch_class_set(pqp_handle *h, const pqp::BatchView &bv, const int *count_v, const int *start_v,
-                            const size_t *smem_v, const int32_t *d_order, cudaStream_t st, int *launches) {
-    int n_cls = 0;
-    for (int v = 0; v < kNumVariants; ++v) n_cls += count_v[v] > 0;
+// Paths a host plan does not launch because their parameter set is out of range: one CTA per order entry writes what a
+// kernel writes for a path it cannot take (PQP_INVALID_PROBLEM, 0 iterations, NaN states).
+__global__ void __launch_bounds__(128)
+pqp_reject_kernel(const __grid_constant__ pqp::BatchView bv, const int32_t *__restrict__ order) {
+    const int b = order[blockIdx.x];
+    const int n = bv.n_points[b], off = bv.offsets[b];
+    if (threadIdx.x == 0) {
+        bv.status[b] = PQP_INVALID_PROBLEM;
+        if (bv.iters) bv.iters[b] = 0;
+    }
+    const double qnan = nan("");
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        pqp_state &o = bv.out_states[off + i];
+        o.x = o.y = o.z = o.k = o.s = qnan;
+        o.v = o.a = 0.0;
+        if (bv.out_frenet) {
+            double *f = bv.out_frenet + 3 * (size_t)(off + i);
+            f[0] = f[1] = f[2] = qnan;
+        }
+    }
+}
+
+// One launch per (set, class) segment g = set * kNumVariants + v with count[g] > 0: count[g] CTAs over the order entries
+// d_order + start[g], with smem[g] bytes and set `set`'s parameters.  A mixed batch has several: they go out on the
+// handle's class lanes (forked from and joined back into `st`), the class of the longest paths first (and inside a class
+// the sets in order), so that the CTAs of the next segment fill the SMs the tail of the previous one leaves idle instead
+// of waiting for its last path.  n_reject > 0: the order entries d_order + reject_start name paths to reject.
+static int launch_class_set(pqp_handle *h, const pqp::BatchView &bv, int n_sets, const int *count, const int *start,
+                            const size_t *smem, const int32_t *d_order, cudaStream_t st, int *launches,
+                            int n_reject = 0, int reject_start = 0) {
+    int n_cls = n_reject > 0;
+    for (int g = 0; g < n_sets * kNumVariants; ++g) n_cls += count[g] > 0;
     const bool fork = n_cls > 1;
     if (fork) PQP_CUDA(cudaEventRecord(h->ev_fork, st));
     int lane = 0, rc = PQP_OK;
-    for (int v = kNumVariants - 1; v >= 0 && rc == PQP_OK; --v) {
-        if (!count_v[v]) continue;
+    for (int v = kNumVariants - 1; v >= 0 && rc == PQP_OK; --v)
+        for (int s = 0; s < n_sets && rc == PQP_OK; ++s) {
+            const int g = s * kNumVariants + v;
+            if (!count[g]) continue;
+            cudaStream_t cs = st;
+            if (fork) {
+                cs = h->cls_stream[lane % PQP_CLASS_LANES];
+                if (lane < PQP_CLASS_LANES) PQP_CUDA(cudaStreamWaitEvent(cs, h->ev_fork, 0));
+                ++lane;
+            }
+            rc = launch_variant(h, v, &h->dsets[s], bv, count[g], d_order + start[g], smem[g], cs);
+            if (rc == PQP_OK && launches) ++*launches;
+        }
+    if (rc == PQP_OK && n_reject > 0) {
         cudaStream_t cs = st;
         if (fork) {
             cs = h->cls_stream[lane % PQP_CLASS_LANES];
             if (lane < PQP_CLASS_LANES) PQP_CUDA(cudaStreamWaitEvent(cs, h->ev_fork, 0));
             ++lane;
         }
-        rc = launch_variant(h, v, bv, count_v[v], d_order + start_v[v], smem_v[v], cs);
-        if (rc == PQP_OK && launches) ++*launches;
+        pqp_reject_kernel<<<n_reject, 128, 0, cs>>>(bv, d_order + reject_start);
+        if (cudaGetLastError() != cudaSuccess) { set_err("pqp_reject_kernel launch failed"); rc = PQP_ERR_CUDA; }
+        else if (launches) ++*launches;
     }
     if (fork)   // join every lane that was used, also after a failed launch: `st` must not run ahead of them
         for (int k = 0; k < std::min(lane, PQP_CLASS_LANES); ++k) {
@@ -245,54 +282,66 @@ static int launch_class_set(pqp_handle *h, const pqp::BatchView &bv, const int *
 }
 
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
-                          const pqp_state *ref, const int32_t *keep_in, cudaStream_t st, int *launches, int form) {
+                          const pqp_state *ref, const int32_t *keep_in, cudaStream_t st, int *launches, int form,
+                          const int32_t *set) {
     static_assert(kNumVariants <= PQP_MAX_VARIANTS, "class plan arrays");
     // keep_control_steps per path
     std::vector<int32_t> keepv((size_t)batch);
     for (int b = 0; b < batch; ++b)
         keepv[b] = form == PQP_FORM_KPC ? 4 : form == PQP_FORM_K ? 1 : keep_in ? keep_in[b] : (n[b] >= 2 ? pqp_keep_control_steps(PQP_FORM_KP, ref + off[b], n[b]) : 1);
-    // The plan (class per path, longest-first order inside a class) only depends on (n, keep): a caller that solves
-    // batches of the same shape back to back reuses it, and the order array already on the device with it.
+    const int n_sets = set ? (int)h->dsets.size() : 1;
+    // The plan (segment per path, longest-first order inside a segment) only depends on (n, keep, set): a caller that
+    // solves batches of the same shape back to back reuses it, and the order array already on the device with it.
     pqp_handle::ClassPlan &pl = h->plan;
     const bool same = pl.valid && pl.form == form && pl.skip == (int)skip_mask() && pl.n.size() == (size_t)batch &&
-                      std::equal(pl.n.begin(), pl.n.end(), n) && pl.keep == keepv;
+                      std::equal(pl.n.begin(), pl.n.end(), n) && pl.keep == keepv && pl.n_sets == n_sets &&
+                      (set ? pl.set.size() == (size_t)batch && std::equal(pl.set.begin(), pl.set.end(), set) : pl.set.empty());
     if (!same) {
         // the pinned order array may still be the source of an earlier asynchronous upload
         PQP_CUDA(cudaStreamSynchronize(st));
         if (pl.stream && pl.stream != st) PQP_CUDA(cudaStreamSynchronize(pl.stream));
         pl.valid = false;
-        std::vector<int> cls((size_t)batch);
-        for (int v = 0; v < kNumVariants; ++v) { pl.count_v[v] = 0; pl.smem_v[v] = 0; }
+        const int G = n_sets * kNumVariants;   // segment G: the rejected paths
+        std::vector<int> seg((size_t)batch);
+        pl.count.assign((size_t)G + 1, 0);
+        pl.start.assign((size_t)G + 2, 0);
+        pl.smem.assign((size_t)G + 1, 0);
         for (int b = 0; b < batch; ++b) {
+            const int s = set ? set[b] : 0;
+            if (s < 0 || s >= n_sets) { seg[b] = G; pl.count[G]++; continue; }
             int v;
             size_t need;
             class_for(h, n[b], keepv[b], &v, &need, form);
-            cls[b] = v;
-            pl.smem_v[v] = std::max(pl.smem_v[v], need);
-            pl.count_v[v]++;
+            seg[b] = s * kNumVariants + v;
+            pl.smem[seg[b]] = std::max(pl.smem[seg[b]], need);
+            pl.count[seg[b]]++;
         }
-        pl.start_v[0] = 0;
-        for (int v = 0; v < kNumVariants; ++v) pl.start_v[v + 1] = pl.start_v[v] + pl.count_v[v];
-        int fill[kNumVariants];
-        for (int v = 0; v < kNumVariants; ++v) fill[v] = pl.start_v[v];
-        for (int b = 0; b < batch; ++b) h->h_order[fill[cls[b]]++] = b;
+        for (int g = 0; g <= G; ++g) pl.start[g + 1] = pl.start[g] + pl.count[g];
+        std::vector<int> fill(pl.start.begin(), pl.start.end() - 1);
+        for (int b = 0; b < batch; ++b) h->h_order[fill[seg[b]]++] = b;
         // longest first; with a hint (pqp_set_order_hint) longest EXPECTED WORK first: stations x expected iterations
         const bool hinted = h->order_hint.size() == (size_t)batch;
         const int32_t *hint = h->order_hint.data();
-        for (int v = 0; v < kNumVariants; ++v)
-            std::stable_sort(h->h_order + pl.start_v[v], h->h_order + pl.start_v[v + 1], [&](int a, int b) {
+        for (int g = 0; g < G; ++g)
+            std::stable_sort(h->h_order + pl.start[g], h->h_order + pl.start[g + 1], [&](int a, int b) {
                 if (hinted) return (long long)n[a] * hint[a] > (long long)n[b] * hint[b];
                 return n[a] > n[b];
             });
         PQP_CUDA(cudaMemcpyAsync(h->d_order, h->h_order, (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
         pl.n.assign(n, n + batch);
         pl.keep = keepv;
+        if (set) pl.set.assign(set, set + batch);
+        else pl.set.clear();
+        pl.n_sets = n_sets;
+        pl.n_reject = pl.count[G];
         pl.skip = (int)skip_mask();
         pl.form = form;
         pl.stream = st;
         pl.valid = true;
     }
-    return launch_class_set(h, bv, pl.count_v, pl.start_v, pl.smem_v, h->d_order, st, launches);
+    const int G = n_sets * kNumVariants;
+    return launch_class_set(h, bv, n_sets, pl.count.data(), pl.start.data(), pl.smem.data(), h->d_order, st, launches,
+                            pl.n_reject, pl.start[G]);
 }
 
 // ---- class selection on the device -------------------------------------------------------------------------------
@@ -317,7 +366,10 @@ struct DispatchArgs {
     int32_t *status, *iters;   // [batch + 1] what the launches write into (copied to the caller's afterwards)
     int32_t *n_view;           // [batch + 1] station counts the launches read: n_points, then 0
     int32_t *key;              // [batch] histogram bucket of every path, -1: outside the bounds
-    int32_t *order;            // [nv][batch] order segments, pre-filled with `batch`
+    int32_t *order;            // [n_sets][nv][batch] order segments, pre-filled with `batch`
+    const int32_t *set;        // [batch] parameter set of every path, NULL: set 0
+    int n_sets;                // sets launched: a path whose set lies outside [0, n_sets) is answered here; 1 without `set`
+    int32_t *hist;             // [n_sets * nv * ncols + n_sets * nv] histogram and bases in global memory, NULL: shared
 };
 
 __global__ void pqp_fill_kernel(int32_t *p, size_t n, int32_t value) {
@@ -326,9 +378,12 @@ __global__ void pqp_fill_kernel(int32_t *p, size_t n, int32_t value) {
 
 __global__ void __launch_bounds__(kDispatchThreads)
 pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
-    extern __shared__ int32_t hist[];   // [nv * ncols] paths per (class, longest-first length bucket), then [nv] bases
+    // [n_sets * nv * ncols] paths per (set, class, longest-first length bucket), then [n_sets * nv] bases: in shared
+    // memory for one set, in global memory (a.hist) for several
+    extern __shared__ int32_t hist_s[];
     __shared__ int32_t warp_sum[kDispatchThreads / 32];
-    const int nb = a.nv * a.ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    int32_t *hist = a.hist ? a.hist : hist_s;
+    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     int32_t *base = hist + nb;
     for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
     if (tid == 0) a.n_view[a.batch] = 0;
@@ -336,11 +391,13 @@ pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
     for (int b = tid; b < a.batch; b += kDispatchThreads) {
         const int n = a.n_points[b], off = a.offsets[b];
         a.n_view[b] = n;
-        const int keep = pqp::keep_control_steps(a.form, a.ref + off, n);
-        const int v = pqp::dispatch_class(a.table, a.ncols, a.form, n, keep, a.max_n, a.min_keep, a.max_keep);
+        const int s = a.set ? a.set[b] : 0;
+        const bool set_ok = s >= 0 && s < a.n_sets;
+        const int keep = set_ok ? pqp::keep_control_steps(a.form, a.ref + off, n) : 0;
+        const int v = set_ok ? pqp::dispatch_class(a.table, a.ncols, a.form, n, keep, a.max_n, a.min_keep, a.max_keep) : -1;
         int key = -1;
         if (v >= 0) {
-            key = (v - a.v0) * a.ncols + (a.ncols - 1 - min(max(n, 0), a.ncols - 1));
+            key = pqp::dispatch_key(s, v - a.v0, a.nv, a.ncols, n);
             atomicAdd(&hist[key], 1);
         } else {
             a.status[b] = PQP_INVALID_PROBLEM;
@@ -387,7 +444,7 @@ pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
         run += c;
     }
     __syncthreads();
-    for (int r = tid; r < a.nv; r += kDispatchThreads) base[r] = hist[r * a.ncols];
+    for (int r = tid; r < nsv; r += kDispatchThreads) base[r] = hist[r * a.ncols];
     __syncthreads();
     for (int b = tid; b < a.batch; b += kDispatchThreads) {
         const int key = a.key[b];
@@ -431,13 +488,37 @@ void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max
 }  // namespace
 
 int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
-                        int max_keep, cudaStream_t st, int *launches) {
+                        int max_keep, cudaStream_t st, int *launches, const int32_t *d_set, int n_param_sets) {
     dispatch_launches(h, form, max_n, min_keep, max_keep);
     int v0, v1;
     form_range(form, &v0, &v1);
     const int nv = v1 - v0, ncols = h->cls_ncols[form];
-    const size_t n_order = (size_t)nv * batch;
-    pqp_fill_kernel<<<(unsigned)std::min<size_t>((n_order + 255) / 256, 1024), 256, 0, st>>>(h->d_disp_order, n_order, batch);
+    // with a set index: every set below n_param_sets (0: all of them), order segments and histogram in global scratch
+    int n_sets = 1;
+    int32_t *order = h->d_disp_order, *hist = nullptr;
+    if (d_set) {
+        n_sets = (int)h->dsets.size();
+        if (n_param_sets > 0) n_sets = std::min(n_sets, n_param_sets);
+        if (n_sets > h->set_cap) {
+            int cap = 1;
+            while (cap < n_sets) cap *= 2;
+            int ncols_max = 0;
+            for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) ncols_max = std::max(ncols_max, h->cls_ncols[f]);
+            int32_t *o = nullptr, *hs = nullptr;
+            PQP_CUDA(cudaMalloc(&o, (size_t)cap * kNumKp * h->max_batch * sizeof(int32_t)));
+            if (cudaMalloc(&hs, (size_t)cap * kNumKp * (ncols_max + 1) * sizeof(int32_t)) != cudaSuccess) {
+                cudaFree(o);
+                set_err("pqp_launch_dispatch: cudaMalloc of the parameter-set sort scratch failed");
+                return PQP_ERR_CUDA;
+            }
+            if (h->d_set_order) { h->retired.push_back(h->d_set_order); h->retired.push_back(h->d_set_hist); }
+            h->d_set_order = o; h->d_set_hist = hs; h->set_cap = cap;
+        }
+        order = h->d_set_order;
+        hist = h->d_set_hist;
+    }
+    const size_t n_order = (size_t)n_sets * nv * batch;
+    pqp_fill_kernel<<<(unsigned)std::min<size_t>((n_order + 255) / 256, 1024), 256, 0, st>>>(order, n_order, batch);
     PQP_CUDA(cudaGetLastError());
     DispatchArgs a;
     a.table = h->d_cls_table + h->cls_off[form];
@@ -445,24 +526,27 @@ int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int b
     a.max_n = max_n; a.min_keep = min_keep; a.max_keep = max_keep; a.batch = batch;
     a.n_points = bv.n_points; a.offsets = bv.offsets; a.ref = bv.ref;
     a.out_states = bv.out_states; a.out_frenet = bv.out_frenet; a.status = h->d_disp_status; a.iters = h->d_disp_iters;
-    a.n_view = h->d_disp_n; a.key = h->d_disp_key; a.order = h->d_disp_order;
-    pqp_dispatch_kernel<<<1, kDispatchThreads, dispatch_smem(nv, ncols), st>>>(a);
+    a.n_view = h->d_disp_n; a.key = h->d_disp_key; a.order = order;
+    a.set = d_set; a.n_sets = n_sets; a.hist = hist;
+    pqp_dispatch_kernel<<<1, kDispatchThreads, hist ? 0 : dispatch_smem(nv, ncols), st>>>(a);
     PQP_CUDA(cudaGetLastError());
     if (launches) *launches += 2;
     pqp::BatchView dv = bv;
     dv.n_points = h->d_disp_n; dv.status = h->d_disp_status; dv.iters = h->d_disp_iters;
-    // Grid per class: `batch` CTAs, or fewer when the class's shortest path says so (its paths hold at least min_n
-    // stations each, `total` in all); the CTAs past the class's last path find -1 and return.
-    int count_v[kNumVariants] = {}, start_v[kNumVariants + 1] = {};
-    size_t smem_v[kNumVariants] = {};
+    // Grid per (set, class): `batch` CTAs, or fewer when the class's shortest path says so (its paths hold at least min_n
+    // stations each, `total` in all); the CTAs past the segment's last path find the sentinel path and return.
+    std::vector<int> count((size_t)n_sets * kNumVariants, 0), start((size_t)n_sets * kNumVariants, 0);
+    std::vector<size_t> smem((size_t)n_sets * kNumVariants, 0);
     const pqp_handle::DispatchLaunches &d = h->disp;
-    for (int v = v0; v < v1; ++v) {
-        if (!d.reach[v]) continue;
-        count_v[v] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
-        start_v[v] = (v - v0) * batch;
-        smem_v[v] = d.smem[v];
-    }
-    const int rc = launch_class_set(h, dv, count_v, start_v, smem_v, h->d_disp_order, st, launches);
+    for (int s = 0; s < n_sets; ++s)
+        for (int v = v0; v < v1; ++v) {
+            if (!d.reach[v]) continue;
+            const int g = s * kNumVariants + v;
+            count[g] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
+            start[g] = (s * nv + v - v0) * batch;
+            smem[g] = d.smem[v];
+        }
+    const int rc = launch_class_set(h, dv, n_sets, count.data(), start.data(), smem.data(), order, st, launches);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaMemcpyAsync(bv.status, h->d_disp_status, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
     if (bv.iters)
@@ -553,6 +637,8 @@ void pqp_destroy(pqp_handle *h) {
     cudaFree(h->d_max_k); cudaFree(h->d_max_kp);
     cudaFree(h->d_cls_table); cudaFree(h->d_disp_order); cudaFree(h->d_disp_key);
     cudaFree(h->d_disp_n); cudaFree(h->d_disp_status); cudaFree(h->d_disp_iters);
+    cudaFree(h->d_set_order); cudaFree(h->d_set_hist);
+    for (void *p : h->retired) cudaFree(p);
     cudaFreeHost(h->h_off); cudaFreeHost(h->h_order);
     cudaFree(h->d_gen); cudaFreeHost(h->h_gen);
     if (h->env && h->env_free) h->env_free(h->env);
@@ -566,13 +652,21 @@ void pqp_destroy(pqp_handle *h) {
     delete h;
 }
 
-int pqp_set_params(pqp_handle *h, const pqp_params *params) {
-    if (!h || !params) return PQP_ERR_ARG;
-    h->params = *params;
-    h->dprm = pqp::dev_params_from(*params);
+int pqp_set_param_sets(pqp_handle *h, int n_sets, const pqp_params *sets) {
+    if (!h || !sets || n_sets < 1 || n_sets > PQP_MAX_PARAM_SETS) {
+        set_err("pqp_set_param_sets: bad argument (needs a handle and 1..PQP_MAX_PARAM_SETS sets)");
+        return PQP_ERR_ARG;
+    }
+    h->sets.assign(sets, sets + n_sets);
+    h->dsets.resize((size_t)n_sets);
+    for (int s = 0; s < n_sets; ++s) h->dsets[s] = pqp::dev_params_from(sets[s]);
+    h->params = h->sets[0];
+    h->dprm = h->dsets[0];
     h->dprm_gen[0] = h->dprm_gen[1] = h->dprm;
     return PQP_OK;
 }
+
+int pqp_set_params(pqp_handle *h, const pqp_params *params) { return pqp_set_param_sets(h, 1, params); }
 
 int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_batch, int max_total_points) {
     if (!out || !params || max_batch < 1 || max_total_points < 2) {
@@ -750,8 +844,8 @@ int pqp_max_points(pqp_handle *h, int formulation) {
     return best;
 }
 
-static int launch_variant(pqp_handle *h, int v, const pqp::BatchView &bv, int count, const int32_t *d_order,
-                          size_t smem_bytes, cudaStream_t st) {
+static int launch_variant(pqp_handle *h, int v, const pqp::DevParams *prm, const pqp::BatchView &bv, int count,
+                          const int32_t *d_order, size_t smem_bytes, cudaStream_t st) {
     if (smem_bytes > (size_t)h->smem_optin) {
         set_err("path too long for one SM's shared memory");
         return PQP_ERR_UNSUPPORTED;
@@ -761,7 +855,7 @@ static int launch_variant(pqp_handle *h, int v, const pqp::BatchView &bv, int co
     static const size_t force = [] { const char *e = getenv("PQP_FORCE_SMEM"); return e ? (size_t)strtoul(e, nullptr, 0) : (size_t)0; }();
     if (force > smem_bytes) smem_bytes = std::min(force, (size_t)h->smem_optin);
     int smem_doubles = (int)(smem_bytes / sizeof(double));
-    void *args[] = {(void *)&h->dprm, (void *)&bv, (void *)&d_order, (void *)&smem_doubles};
+    void *args[] = {(void *)prm, (void *)&bv, (void *)&d_order, (void *)&smem_doubles};
     PQP_CUDA(cudaLaunchKernel(kVariants[v].fn, dim3(count), dim3(kVariants[v].threads), args, smem_bytes, st));
     return PQP_OK;
 }
@@ -821,7 +915,7 @@ int pqp_solve_batch_device(pqp_handle *h, int formulation, int batch, int total_
         PQP_CUDA(cudaGetLastError());
         order = h->d_order_auto;
     }
-    int rc = launch_variant(h, v, bv, batch, order, smem, st);
+    int rc = launch_variant(h, v, &h->dprm, bv, batch, order, smem, st);
     if (rc != PQP_OK) return rc;
     if (stats) {
         memset(stats, 0, sizeof(*stats));
@@ -885,9 +979,22 @@ int pqp_solve_batch_device_dispatch(pqp_handle *h, int formulation, int batch, i
                                     const double *d_x0, const double *d_end_heading, const double *d_max_k,
                                     const double *d_max_kp, pqp_state *d_out_states, double *d_out_frenet,
                                     int32_t *d_status, int32_t *d_iters, void *stream, pqp_stats *stats) {
-    if (!h || batch < 0 || !d_n_points || !d_offsets || !d_ref || !d_bounds || !d_x0 || !d_end_heading ||
-        !d_out_states || !d_status) {
-        set_err("pqp_solve_batch_device_dispatch: bad argument");
+    return pqp_solve_batch_device_dispatch_sets(h, formulation, batch, total_points, max_n_points, min_keep, max_keep, 0,
+                                                d_n_points, d_offsets, d_ref, d_bounds, d_x0, d_end_heading, d_max_k,
+                                                d_max_kp, nullptr, d_out_states, d_out_frenet, d_status, d_iters, stream,
+                                                stats);
+}
+
+int pqp_solve_batch_device_dispatch_sets(pqp_handle *h, int formulation, int batch, int total_points,
+                                         int max_n_points, int min_keep, int max_keep, int n_param_sets,
+                                         const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                                         const pqp_station_bounds *d_bounds, const double *d_x0,
+                                         const double *d_end_heading, const double *d_max_k, const double *d_max_kp,
+                                         const int32_t *d_param_index, pqp_state *d_out_states, double *d_out_frenet,
+                                         int32_t *d_status, int32_t *d_iters, void *stream, pqp_stats *stats) {
+    if (!h || batch < 0 || n_param_sets < 0 || !d_n_points || !d_offsets || !d_ref || !d_bounds || !d_x0 ||
+        !d_end_heading || !d_out_states || !d_status) {
+        set_err("pqp_solve_batch_device_dispatch(_sets): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
@@ -912,7 +1019,8 @@ int pqp_solve_batch_device_dispatch(pqp_handle *h, int formulation, int batch, i
     bv.max_k = d_max_k; bv.max_kp = d_max_kp;
     if (stats) PQP_CUDA(cudaEventRecord(h->ev[0], st));
     int launches = 0;
-    int rc = pqp_launch_dispatch(h, bv, formulation, batch, total_points, max_n_points, min_keep, max_keep, st, &launches);
+    int rc = pqp_launch_dispatch(h, bv, formulation, batch, total_points, max_n_points, min_keep, max_keep, st, &launches,
+                                 d_param_index, n_param_sets);
     if (rc != PQP_OK) return rc;
     if (stats) {
         memset(stats, 0, sizeof(*stats));
@@ -1074,8 +1182,16 @@ int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_
                     const pqp_station_bounds *bounds, const double *x0, const double *end_heading,
                     const double *max_k, const double *max_kp, pqp_state *out_states, double *out_frenet,
                     int32_t *status, int32_t *iters, pqp_stats *stats) {
+    return pqp_solve_batch_sets(h, formulation, batch, n_points, ref, bounds, x0, end_heading, max_k, max_kp, nullptr,
+                                out_states, out_frenet, status, iters, stats);
+}
+
+int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch, const int32_t *n_points, const pqp_state *ref,
+                         const pqp_station_bounds *bounds, const double *x0, const double *end_heading,
+                         const double *max_k, const double *max_kp, const int32_t *param_index, pqp_state *out_states,
+                         double *out_frenet, int32_t *status, int32_t *iters, pqp_stats *stats) {
     if (!h || batch < 0 || (batch > 0 && (!n_points || !ref || !bounds || !x0 || !end_heading || !out_states || !status))) {
-        set_err("pqp_solve_batch: bad argument");
+        set_err("pqp_solve_batch(_sets): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation != PQP_FORM_KP && formulation != PQP_FORM_K && formulation != PQP_FORM_KPC) {
@@ -1094,14 +1210,26 @@ int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_
     static const bool generic_k = [] { const char *e = getenv("PQP_GENERIC_K"); return e && *e == '1'; }();
     const bool kpc_classes = formulation == PQP_FORM_KPC && !generic_kpc;
     const bool k_classes = formulation == PQP_FORM_K && !generic_k;
-    if (formulation != PQP_FORM_KP && !kpc_classes && !k_classes)
+    if (formulation != PQP_FORM_KP && !kpc_classes && !k_classes) {
+        if (param_index) {
+            set_err("the host-assembled diagnostic path (PQP_GENERIC_K / PQP_GENERIC_KPC) takes no parameter-set index");
+            return PQP_ERR_UNSUPPORTED;
+        }
         return solve_batch_generic(h, formulation, batch, n_points, ref, bounds, x0, end_heading, max_k, max_kp, out_states,
                                    out_frenet, status, iters, stats);
+    }
     if (batch > h->max_batch) {
         set_err("batch exceeds the handle's max_batch");
         return PQP_ERR_CAPACITY;
     }
-    // offsets; shape class and shared-memory need per path
+    if (param_index && h->defer_sync) {
+        set_err("pqp_solve_batch_sets: no parameter-set index on a multi-device handle");
+        return PQP_ERR_UNSUPPORTED;
+    }
+    // offsets; launch segment (set * kNumVariants + shape class) and shared-memory need per path; segment G = the paths
+    // whose set index is out of range (rejected, not launched)
+    const int n_sets = param_index ? (int)h->dsets.size() : 1;
+    const int G = n_sets * kNumVariants;
     long long total = 0;
     h->h_off[0] = 0;
     std::vector<int> cls((size_t)batch);
@@ -1112,11 +1240,13 @@ int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_
         total += n;
         if (total > h->max_total) { set_err("station count exceeds the handle's max_total_points"); return PQP_ERR_CAPACITY; }
         h->h_off[b + 1] = (int32_t)total;
+        const int s = param_index ? param_index[b] : 0;
+        if (s < 0 || s >= n_sets) { cls[b] = G; need_b[b] = 0; continue; }
         const int keep = (n >= 2) ? pqp_keep_control_steps(formulation, ref + h->h_off[b], n) : 1;
         int v;
         size_t need;
         class_for(h, n, keep, &v, &need, formulation);
-        cls[b] = v;
+        cls[b] = s * kNumVariants + v;
         need_b[b] = need;
     }
     // The batch is cut into contiguous chunks of paths that are pipelined over two streams: the
@@ -1141,26 +1271,27 @@ int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_
             okey[b] = n >= 1 ? order_key(n, x0[3 * (size_t)b], bounds[h->h_off[b]].c0_lb, bounds[h->h_off[b]].c0_ub) : 0.0;
         }
     }
-    // per chunk: per-class longest-first order (written into the pinned order array at the chunk's range)
-    int count_cv[kMaxChunks][kNumVariants];
-    int start_cv[kMaxChunks][kNumVariants + 1];
-    size_t smem_cv[kMaxChunks][kNumVariants];
+    // per chunk: per-segment longest-first order (written into the pinned order array at the chunk's range), the
+    // rejected paths last
+    std::vector<int> count_cv((size_t)n_chunks * (G + 1)), start_cv((size_t)n_chunks * (G + 2));
+    std::vector<size_t> smem_cv((size_t)n_chunks * (G + 1));
     for (int k = 0; k < n_chunks; ++k) {
-        for (int v = 0; v < kNumVariants; ++v) { count_cv[k][v] = 0; smem_cv[k][v] = 0; }
+        int *count_k = count_cv.data() + (size_t)k * (G + 1), *start_k = start_cv.data() + (size_t)k * (G + 2);
+        size_t *smem_k = smem_cv.data() + (size_t)k * (G + 1);
+        for (int g = 0; g <= G; ++g) { count_k[g] = 0; smem_k[g] = 0; }
         for (int b = cb[k]; b < cb[k + 1]; ++b) {
-            count_cv[k][cls[b]]++;
-            smem_cv[k][cls[b]] = std::max(smem_cv[k][cls[b]], need_b[b]);
+            count_k[cls[b]]++;
+            smem_k[cls[b]] = std::max(smem_k[cls[b]], need_b[b]);
         }
-        start_cv[k][0] = cb[k];
-        for (int v = 0; v < kNumVariants; ++v) start_cv[k][v + 1] = start_cv[k][v] + count_cv[k][v];
-        int fill[kNumVariants];
-        for (int v = 0; v < kNumVariants; ++v) fill[v] = start_cv[k][v];
+        start_k[0] = cb[k];
+        for (int g = 0; g <= G; ++g) start_k[g + 1] = start_k[g] + count_k[g];
+        std::vector<int> fill(start_k, start_k + G + 1);
         for (int b = cb[k]; b < cb[k + 1]; ++b) h->h_order[fill[cls[b]]++] = b;
         const bool hinted = h->order_hint.size() == (size_t)batch;
         const int32_t *hint = h->order_hint.data();
         const bool keyed = !hinted && auto_order_enabled() && batch <= kAutoOrderMax;   // as pqp_order_kernel does on the device
-        for (int v = 0; v < kNumVariants; ++v)
-            std::stable_sort(h->h_order + start_cv[k][v], h->h_order + start_cv[k][v + 1], [&](int a, int b) {
+        for (int g = 0; g < G; ++g)
+            std::stable_sort(h->h_order + start_k[g], h->h_order + start_k[g + 1], [&](int a, int b) {
                 if (hinted) return (long long)n_points[a] * hint[a] > (long long)n_points[b] * hint[b];
                 if (keyed) return okey[a] > okey[b];
                 return n_points[a] > n_points[b];
@@ -1233,23 +1364,38 @@ int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_
             PQP_CUDA_DRAIN(cudaMemcpyAsync(h->d_max_kp + o0, max_kp + o0, nT * sizeof(double), cudaMemcpyHostToDevice, st));
         }
         if (!ev1_done) { PQP_CUDA_DRAIN(cudaEventRecord(h->ev[1], st)); ev1_done = true; }
-        // One launch per class of the chunk; a mixed-length chunk has several: they go out on the class lanes (forked
-        // after the chunk's upload, joined before its download), longest class first, so that they overlap instead of
-        // each waiting for the tail of the one before.
+        // One launch per segment of the chunk (and one for its rejected paths); a mixed-length chunk has several: they go
+        // out on the class lanes (forked after the chunk's upload, joined before its download), longest class first, so
+        // that they overlap instead of each waiting for the tail of the one before.
+        const int *count_k = count_cv.data() + (size_t)k * (G + 1), *start_k = start_cv.data() + (size_t)k * (G + 2);
+        const size_t *smem_k = smem_cv.data() + (size_t)k * (G + 1);
         int n_cls = 0;
-        for (int v = 0; v < kNumVariants; ++v) n_cls += count_cv[k][v] > 0;
+        for (int g = 0; g <= G; ++g) n_cls += count_k[g] > 0;
         if (n_cls > 1) PQP_CUDA_DRAIN(cudaEventRecord(h->ev_fork, st));
         int lane = 0;
-        for (int v = kNumVariants - 1; v >= 0; --v) {
-            if (!count_cv[k][v]) continue;
+        for (int v = kNumVariants - 1; v >= 0; --v)
+            for (int s = 0; s < n_sets; ++s) {
+                const int g = s * kNumVariants + v;
+                if (!count_k[g]) continue;
+                cudaStream_t cs = st;
+                if (n_cls > 1) {
+                    cs = h->cls_stream[lane % PQP_CLASS_LANES];
+                    PQP_CUDA_DRAIN(cudaStreamWaitEvent(cs, h->ev_fork, 0));
+                    ++lane;
+                }
+                int rc = launch_variant(h, v, &h->dsets[s], bv, count_k[g], h->d_order + start_k[g], smem_k[g], cs);
+                if (rc != PQP_OK) { drain(); return rc; }
+                ++launches;
+            }
+        if (count_k[G]) {
             cudaStream_t cs = st;
             if (n_cls > 1) {
                 cs = h->cls_stream[lane % PQP_CLASS_LANES];
                 PQP_CUDA_DRAIN(cudaStreamWaitEvent(cs, h->ev_fork, 0));
                 ++lane;
             }
-            int rc = launch_variant(h, v, bv, count_cv[k][v], h->d_order + start_cv[k][v], smem_cv[k][v], cs);
-            if (rc != PQP_OK) { drain(); return rc; }
+            pqp_reject_kernel<<<count_k[G], 128, 0, cs>>>(bv, h->d_order + start_k[G]);
+            PQP_CUDA_DRAIN(cudaGetLastError());
             ++launches;
         }
         for (int j = 0; j < std::min(lane, PQP_CLASS_LANES); ++j) {

@@ -50,4 +50,12 @@ PQP_HD int dispatch_class(const int8_t *table, int ncols, int formulation, int n
     return table[row * ncols + col];
 }
 
+// Sort key of the device dispatch for a path of n stations on class `cls` (0-based within the formulation's nv classes)
+// with parameter set `set`: histogram bucket (set * nv + cls) * ncols + the longest-first length bucket.  The order
+// segment of the path is key / ncols = set * nv + cls, and ascending keys inside it run from the longest path down.
+PQP_HD int dispatch_key(int set, int cls, int nv, int ncols, int n) {
+    const int col = n < 0 ? 0 : (n >= ncols ? ncols - 1 : n);
+    return (set * nv + cls) * ncols + (ncols - 1 - col);
+}
+
 }  // namespace pqp

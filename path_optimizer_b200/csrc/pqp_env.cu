@@ -22,6 +22,8 @@ namespace {
 using pqp::CarCircles;
 using pqp::MapTable;
 using pqp::MapView;
+using pqp::ParamRow;
+using pqp::ParamTable;
 using pqp::SplineView;
 
 struct EnvState {
@@ -36,6 +38,7 @@ struct EnvState {
     // per-batch scratch (sized from the handle's capacity at first use)
     int32_t *d_nvalid = nullptr, *d_nkept = nullptr, *d_ok = nullptr, *d_koff = nullptr;
     int32_t *d_mapidx = nullptr;   // pqp_plan_batch_maps: the uploaded map index
+    int32_t *d_setidx = nullptr;   // pqp_plan_batch_sets: the uploaded parameter-set index
     double *d_spl = nullptr;       // densify workspace: 13 doubles per station
     pqp_state *d_dense = nullptr;  // densify output [batch][max_out] (grow-only)
     size_t dense_cap = 0;
@@ -50,7 +53,7 @@ struct EnvState {
 
 void env_free(void *p) {
     EnvState *e = (EnvState *)p;
-    cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx);
+    cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx); cudaFree(e->d_setidx);
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
     cudaFree(e->d_tmp);
@@ -71,6 +74,7 @@ int env_get(pqp_handle *h, EnvState **out) {
         PQP_CUDA(cudaMalloc(&e->d_ok, B * sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_koff, (B + 1) * sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_mapidx, B * sizeof(int32_t)));
+        PQP_CUDA(cudaMalloc(&e->d_setidx, B * sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_nmaps, sizeof(int32_t)));
         PQP_CUDA(cudaMemset(e->d_nmaps, 0, sizeof(int32_t)));
         PQP_CUDA(cudaMalloc(&e->d_spl, T * 13 * sizeof(double)));
@@ -95,10 +99,14 @@ int grow(T **p, size_t *cap, size_t need_bytes) {
 // kernels
 // ---------------------------------------------------------------------------------------------
 
-struct BoundsArgs {
+// The env kernels take the handle's parameter sets by value (pqp::ParamTable): R = 1 row (set 0) for the entries without
+// a set index, kSetRows with one.
+constexpr int kSetRows = PQP_MAX_PARAM_SETS;
+static_assert(sizeof(ParamTable<kSetRows>) + 512 <= 32764, "the parameter table must fit a kernel's parameter space");
+
+template <int R> struct BoundsArgs {
     MapTable maps;
-    double radius;
-    double d[4];
+    ParamTable<R> prm;
     int mode;
     const int32_t *n_points, *offsets;
     const pqp_state *ref;
@@ -110,15 +118,17 @@ struct BoundsArgs {
 };
 
 // grid (ceil(4*maxN/128), batch): thread = (station, circle) of path blockIdx.y
+template <int R>
 __global__ void __launch_bounds__(128)
-pqp_bounds_kernel(const __grid_constant__ BoundsArgs a) {
+pqp_bounds_kernel(const __grid_constant__ BoundsArgs<R> a) {
     const int b = a.first_path + blockIdx.y;
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     const int i = t >> 2, j = t & 3;
     const int n = a.n_points[b];
     if (i >= n) return;
     const MapView *mp = pqp::map_of(a.maps, b);
-    if (!mp) {                     // map index outside the set: no usable station, the QP reports PQP_INVALID_PROBLEM
+    const ParamRow *pr = pqp::param_of(a.prm, b);
+    if (!mp || !pr) {              // map or set index outside its set: no usable station, the QP reports PQP_INVALID_PROBLEM
         if (t == 0) a.n_valid[b] = 0;
         return;
     }
@@ -132,7 +142,7 @@ pqp_bounds_kernel(const __grid_constant__ BoundsArgs a) {
         ys = SplineView{nk, a.knots + k0, a.yc + 4 * (size_t)k0};
     }
     double ub, lb;
-    const bool blocked = pqp::circle_bounds(map, a.radius, a.mode, st, a.d[j], xs, ys, ub, lb);
+    const bool blocked = pqp::circle_bounds(map, pr->radius, a.mode, st, pr->d[j], xs, ys, ub, lb);
     double *o = &a.out[off + i].c0_ub + 2 * j;
     o[0] = ub;
     o[1] = lb;
@@ -155,11 +165,11 @@ __global__ void pqp_check_states_kernel(const MapView *maps, const __grid_consta
     ok[i] = pqp::state_collision_free(map, car, s[i].x, s[i].y, s[i].z) ? 1 : 0;
 }
 
-// The tails look their path's map up once per CTA (thread 0, into shared memory).  Without a collision check the map
-// is not read at all, and no map set is needed.
-struct TailArgs {
+// The tails look their path's map and parameter set up once per CTA (thread 0, into shared memory).  Without a
+// collision check neither is read, and no map set is needed.
+template <int R> struct TailArgs {
     MapTable maps;
-    CarCircles car;
+    ParamTable<R> prm;
     const int32_t *n_points, *offsets;
     const int32_t *status;   // optional: tail only for PQP_SOLVED paths (plan chain)
     pqp_state *paths;
@@ -169,9 +179,10 @@ struct TailArgs {
 
 // Raw tail (path_optimizer.cpp:191-202): one CTA per path.  Thread 0 re-accumulates s in the
 // reference's serial order while every thread checks footprints; the cut is the first failure.
+template <int R>
 __global__ void __launch_bounds__(128)
-pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
-    __shared__ int first_fail, has_map;
+pqp_finish_raw_kernel(const __grid_constant__ TailArgs<R> a) {
+    __shared__ int first_fail, has_map, row_s;
     __shared__ MapView map_s;
     const int b = blockIdx.x;
     const int n = a.n_points[b];
@@ -183,18 +194,21 @@ pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
     if (threadIdx.x == 0) {
         first_fail = n;
         const MapView *mp = a.collision_check ? pqp::map_of(a.maps, b) : nullptr;
-        has_map = mp != nullptr;
+        const ParamRow *pr = a.collision_check ? pqp::param_of(a.prm, b) : nullptr;
+        has_map = mp != nullptr && pr != nullptr;
         map_s = mp ? *mp : MapView{};
+        row_s = pr ? (int)(pr - a.prm.row) : 0;
     }
     __syncthreads();
-    if (a.collision_check && !has_map) {   // map index outside the set
+    if (a.collision_check && !has_map) {   // map or set index outside its set
         if (threadIdx.x == 0) { a.n_kept[b] = 0; a.ok[b] = 0; }
         return;
     }
     if (a.collision_check) {
         const MapView map = map_s;
+        const CarCircles &car = a.prm.row[row_s].car;
         for (int i = threadIdx.x; i < n; i += blockDim.x)
-            if (!pqp::state_collision_free(map, a.car, p[i].x, p[i].y, p[i].z)) atomicMin(&first_fail, i);
+            if (!pqp::state_collision_free(map, car, p[i].x, p[i].y, p[i].z)) atomicMin(&first_fail, i);
     }
     if (threadIdx.x == 0) {
         pqp::accumulate_s(n, p);
@@ -207,9 +221,9 @@ pqp_finish_raw_kernel(const __grid_constant__ TailArgs a) {
     }
 }
 
-struct DensifyArgs {
+template <int R> struct DensifyArgs {
     MapTable maps;
-    CarCircles car;
+    ParamTable<R> prm;
     const int32_t *n_points, *offsets, *status;
     const pqp_state *paths;
     double *ws;              // 13 doubles per station: t, x/y coef (4 each), 4 scratch
@@ -221,9 +235,10 @@ struct DensifyArgs {
 
 // Densifying tail (path_optimizer.cpp:203-230): one CTA per path; threads 0 and 32 fit x(s), y(s),
 // then all threads evaluate / check the samples.
+template <int R>
 __global__ void __launch_bounds__(128)
-pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
-    __shared__ int first_fail, has_map, knots_ok;
+pqp_densify_kernel(const __grid_constant__ DensifyArgs<R> a) {
+    __shared__ int first_fail, has_map, knots_ok, row_s;
     __shared__ MapView map_s;
     const int b = blockIdx.x;
     const int n = a.n_points[b];
@@ -240,15 +255,18 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
     if (threadIdx.x == 0) {
         first_fail = 0x7fffffff;
         const MapView *mp = a.collision_check ? pqp::map_of(a.maps, b) : nullptr;
-        has_map = mp != nullptr;
+        const ParamRow *pr = a.collision_check ? pqp::param_of(a.prm, b) : nullptr;
+        has_map = mp != nullptr && pr != nullptr;
         map_s = mp ? *mp : MapView{};
+        row_s = pr ? (int)(pr - a.prm.row) : 0;
     }
     __syncthreads();
-    if (a.collision_check && !has_map) {   // map index outside the set
+    if (a.collision_check && !has_map) {   // map or set index outside its set
         if (threadIdx.x == 0) { a.n_out[b] = 0; a.ok[b] = 0; }
         return;
     }
     const MapView map = map_s;
+    const CarCircles &car = a.prm.row[row_s].car;
     // threads 0 and 32 fit x(s) and y(s) side by side (diag / rhs scratch: 2n doubles each)
     if (threadIdx.x == 0) {
         knots_ok = pqp::knots_increasing(n, t);
@@ -272,7 +290,7 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs a) {
     const long long lim = cnt < (long long)a.max_out + 1 ? cnt : (long long)a.max_out + 1;   // samples that matter
     for (long long i = threadIdx.x; i < lim; i += blockDim.x) {
         const pqp_state st = pqp::densify_sample(xs, ys, pqp::mul((double)i, a.spacing));
-        if (a.collision_check && !pqp::state_collision_free(map, a.car, st.x, st.y, st.z)) atomicMin(&first_fail, (int)i);
+        if (a.collision_check && !pqp::state_collision_free(map, car, st.x, st.y, st.z)) atomicMin(&first_fail, (int)i);
         if (i < a.max_out) out[i] = st;
     }
     __syncthreads();
@@ -374,12 +392,29 @@ PathsView handle_paths(pqp_handle *h, EnvState *e) {
     return PathsView{h->d_n, h->d_off, h->d_ref, e->d_koff, e->d_knots, e->d_xc, e->d_yc};
 }
 
-int launch_bounds_kernel(pqp_handle *h, EnvState *e, int mode, int batch, int max_n, const PathsView &p,
-                         const int32_t *map_index, pqp_station_bounds *out, cudaStream_t st) {
-    BoundsArgs a;
+// The handle's first n_sets parameter sets for the kernels; `index` [batch] on the device, or NULL for set 0.
+template <int R> ParamTable<R> param_table(const pqp_handle *h, const int32_t *index, int n_sets) {
+    ParamTable<R> t;
+    t.n = n_sets;
+    t.index = index;
+    for (int s = 0; s < n_sets; ++s) t.row[s] = pqp::make_param_row(h->sets[s]);
+    return t;
+}
+
+// A stage's parameter sets: the path index on the device (NULL: set 0 for every path, one row) and the number of sets
+// an index may name.
+struct SetIndex {
+    const int32_t *index;
+    int n_sets;
+};
+constexpr SetIndex kSet0{nullptr, 1};
+
+template <int R>
+int launch_bounds_impl(pqp_handle *h, EnvState *e, int mode, int batch, int max_n, const PathsView &p,
+                       const int32_t *map_index, SetIndex set, pqp_station_bounds *out, cudaStream_t st) {
+    BoundsArgs<R> a;
     a.maps = map_table(e, map_index);
-    a.radius = h->params.circle_radius;
-    a.d[0] = h->params.d1; a.d[1] = h->params.d2; a.d[2] = h->params.d3; a.d[3] = h->params.d4;
+    a.prm = param_table<R>(h, set.index, set.n_sets);
     a.mode = mode;
     a.n_points = p.n_points; a.offsets = p.offsets; a.ref = p.ref;
     a.koff = p.koff; a.knots = p.knots; a.xc = p.xc; a.yc = p.yc;
@@ -389,10 +424,39 @@ int launch_bounds_kernel(pqp_handle *h, EnvState *e, int mode, int batch, int ma
     for (int first = 0; max_n > 0 && first < batch; first += 65535) {
         a.first_path = first;
         dim3 grid((unsigned)((4 * max_n + 127) / 128), (unsigned)std::min(65535, batch - first));
-        pqp_bounds_kernel<<<grid, 128, 0, st>>>(a);
+        pqp_bounds_kernel<R><<<grid, 128, 0, st>>>(a);
         PQP_CUDA(cudaGetLastError());
     }
     return PQP_OK;
+}
+
+int launch_bounds_kernel(pqp_handle *h, EnvState *e, int mode, int batch, int max_n, const PathsView &p,
+                         const int32_t *map_index, SetIndex set, pqp_station_bounds *out, cudaStream_t st) {
+    return set.index ? launch_bounds_impl<kSetRows>(h, e, mode, batch, max_n, p, map_index, set, out, st)
+                     : launch_bounds_impl<1>(h, e, mode, batch, max_n, p, map_index, kSet0, out, st);
+}
+
+template <int R>
+int launch_finish_raw_impl(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
+                           const int32_t *d_status, const int32_t *map_index, SetIndex set, pqp_state *d_paths,
+                           int collision_check, int32_t *d_n_kept, int32_t *d_ok, cudaStream_t st) {
+    TailArgs<R> a;
+    a.maps = map_table(e, map_index); a.prm = param_table<R>(h, set.index, set.n_sets);
+    a.n_points = d_n; a.offsets = d_off; a.status = d_status; a.paths = d_paths;
+    a.collision_check = collision_check ? 1 : 0;
+    a.n_kept = d_n_kept; a.ok = d_ok;
+    pqp_finish_raw_kernel<R><<<batch, 128, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    return PQP_OK;
+}
+
+int launch_finish_raw(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
+                      const int32_t *d_status, const int32_t *map_index, SetIndex set, pqp_state *d_paths,
+                      int collision_check, int32_t *d_n_kept, int32_t *d_ok, cudaStream_t st) {
+    return set.index ? launch_finish_raw_impl<kSetRows>(h, e, batch, d_n, d_off, d_status, map_index, set, d_paths,
+                                                        collision_check, d_n_kept, d_ok, st)
+                     : launch_finish_raw_impl<1>(h, e, batch, d_n, d_off, d_status, map_index, kSet0, d_paths,
+                                                 collision_check, d_n_kept, d_ok, st);
 }
 
 }  // namespace
@@ -529,7 +593,7 @@ int pqp_update_bounds_batch(pqp_handle *h, int mode, int batch, const int32_t *n
     rc = upload_paths(h, e, batch, n_points, ref, mode, n_knots, knots, x_coef, y_coef, &total, &max_n, &h2d, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
-    rc = launch_bounds_kernel(h, e, mode, batch, max_n, handle_paths(h, e), nullptr, h->d_bounds, st);
+    rc = launch_bounds_kernel(h, e, mode, batch, max_n, handle_paths(h, e), nullptr, kSet0, h->d_bounds, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[2], st));
     PQP_CUDA(cudaMemcpyAsync(out_bounds, h->d_bounds, (size_t)total * sizeof(pqp_station_bounds), cudaMemcpyDeviceToHost, st));
@@ -570,6 +634,39 @@ __global__ void pqp_limits_kernel(double mu, double rate, double kmax, int from_
     if (i >= n) return;
     if (from_spline) { max_k[i] = kmax; max_kp[i] = 1.7976931348623157e308; return; }
     limits_of(mu, rate, ref[i].v, ref[i].a, max_k + i, max_kp + i);
+}
+
+// The same limits with a parameter set per path (plan chain with a set index): grid (ceil(maxN/128), batch), thread =
+// station of path blockIdx.y, looking its row up once.  A path whose set is out of range is skipped (it is not solved).
+struct LimitsArgs {
+    ParamTable<kSetRows> prm;
+    const int32_t *n_points, *offsets;
+    const pqp_state *ref;
+    double *max_k, *max_kp;
+    int first_path;
+};
+__global__ void __launch_bounds__(128)
+pqp_limits_sets_kernel(const __grid_constant__ LimitsArgs a) {
+    const int b = a.first_path + blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_points[b]) return;
+    const ParamRow *pr = pqp::param_of(a.prm, b);
+    if (!pr) return;
+    const int s = a.offsets[b] + i;
+    limits_of(pr->mu, pr->rate, a.ref[s].v, a.ref[s].a, a.max_k + s, a.max_kp + s);
+}
+
+static int launch_limits_sets(pqp_handle *h, int batch, int max_n, const int32_t *d_n, const int32_t *d_off,
+                              const pqp_state *d_ref, SetIndex set, double *d_max_k, double *d_max_kp, cudaStream_t st) {
+    LimitsArgs a;
+    a.prm = param_table<kSetRows>(h, set.index, set.n_sets);
+    a.n_points = d_n; a.offsets = d_off; a.ref = d_ref; a.max_k = d_max_k; a.max_kp = d_max_kp;
+    for (int first = 0; max_n > 0 && first < batch; first += 65535) {
+        a.first_path = first;
+        pqp_limits_sets_kernel<<<dim3((unsigned)((max_n + 127) / 128), (unsigned)std::min(65535, batch - first)), 128, 0, st>>>(a);
+        PQP_CUDA(cudaGetLastError());
+    }
+    return PQP_OK;
 }
 
 int pqp_update_limits(const pqp_params *params, int from_spline, int n, const pqp_state *ref, double *max_k, double *max_kp) {
@@ -636,13 +733,9 @@ int pqp_finish_raw_batch(pqp_handle *h, int batch, const int32_t *n_points, pqp_
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaMemcpyAsync(h->d_out, h->d_ref, (size_t)total * sizeof(pqp_state), cudaMemcpyDeviceToDevice, st));
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
-    TailArgs a;
-    a.maps = map_table(e, nullptr); a.car = pqp::make_car_circles(h->params);
-    a.n_points = h->d_n; a.offsets = h->d_off; a.status = nullptr; a.paths = h->d_out;
-    a.collision_check = collision_check ? 1 : 0;
-    a.n_kept = e->d_nkept; a.ok = e->d_ok;
-    pqp_finish_raw_kernel<<<batch, 128, 0, st>>>(a);
-    PQP_CUDA(cudaGetLastError());
+    rc = launch_finish_raw(h, e, batch, h->d_n, h->d_off, nullptr, nullptr, kSet0, h->d_out, collision_check, e->d_nkept,
+                           e->d_ok, st);
+    if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[2], st));
     PQP_CUDA(cudaMemcpyAsync(paths, h->d_out, (size_t)total * sizeof(pqp_state), cudaMemcpyDeviceToHost, st));
     PQP_CUDA(cudaMemcpyAsync(out_n_kept, e->d_nkept, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -660,19 +753,34 @@ int pqp_finish_raw_batch(pqp_handle *h, int batch, const int32_t *n_points, pqp_
     return PQP_OK;
 }
 
-static int launch_densify(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
-                          const int32_t *d_status, const int32_t *d_map_index, const pqp_state *d_paths, double spacing,
-                          int collision_check, int max_out, pqp_state *d_out, int32_t *d_n_out, int32_t *d_ok,
-                          cudaStream_t st) {
-    DensifyArgs a;
-    a.maps = map_table(e, d_map_index); a.car = pqp::make_car_circles(h->params);
+}  // extern "C"
+
+template <int R>
+static int launch_densify_impl(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
+                               const int32_t *d_status, const int32_t *d_map_index, SetIndex set, const pqp_state *d_paths,
+                               double spacing, int collision_check, int max_out, pqp_state *d_out, int32_t *d_n_out,
+                               int32_t *d_ok, cudaStream_t st) {
+    DensifyArgs<R> a;
+    a.maps = map_table(e, d_map_index); a.prm = param_table<R>(h, set.index, set.n_sets);
     a.n_points = d_n; a.offsets = d_off; a.status = d_status; a.paths = d_paths;
     a.ws = e->d_spl; a.spacing = spacing; a.collision_check = collision_check ? 1 : 0; a.max_out = max_out;
     a.out = d_out; a.n_out = d_n_out; a.ok = d_ok;
-    pqp_densify_kernel<<<batch, 128, 0, st>>>(a);
+    pqp_densify_kernel<R><<<batch, 128, 0, st>>>(a);
     PQP_CUDA(cudaGetLastError());
     return PQP_OK;
 }
+
+static int launch_densify(pqp_handle *h, EnvState *e, int batch, const int32_t *d_n, const int32_t *d_off,
+                          const int32_t *d_status, const int32_t *d_map_index, SetIndex set, const pqp_state *d_paths,
+                          double spacing, int collision_check, int max_out, pqp_state *d_out, int32_t *d_n_out,
+                          int32_t *d_ok, cudaStream_t st) {
+    return set.index ? launch_densify_impl<kSetRows>(h, e, batch, d_n, d_off, d_status, d_map_index, set, d_paths, spacing,
+                                                     collision_check, max_out, d_out, d_n_out, d_ok, st)
+                     : launch_densify_impl<1>(h, e, batch, d_n, d_off, d_status, d_map_index, kSet0, d_paths, spacing,
+                                              collision_check, max_out, d_out, d_n_out, d_ok, st);
+}
+
+extern "C" {
 
 int pqp_densify_batch(pqp_handle *h, int batch, const int32_t *n_points, const pqp_state *paths, double output_spacing,
                       int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
@@ -697,7 +805,7 @@ int pqp_densify_batch(pqp_handle *h, int batch, const int32_t *n_points, const p
     PQP_CUDA(cudaEventRecord(e->ev[1], st));
     rc = grow(&e->d_dense, &e->dense_cap, (size_t)batch * (size_t)max_out * sizeof(pqp_state));
     if (rc != PQP_OK) return rc;
-    rc = launch_densify(h, e, batch, h->d_n, h->d_off, nullptr, nullptr, h->d_ref, output_spacing, collision_check,
+    rc = launch_densify(h, e, batch, h->d_n, h->d_off, nullptr, nullptr, kSet0, h->d_ref, output_spacing, collision_check,
                         max_out, e->d_dense, e->d_nkept, e->d_ok, st);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaEventRecord(e->ev[2], st));
@@ -726,6 +834,8 @@ struct ChainIO {
     size_t total;
     PathsView paths;
     const int32_t *map_index;       // [batch] map of every path (bounds and collision check), NULL: map 0
+    SetIndex set;                   // parameter set of every path (device index, NULL: set 0) and the sets it may name
+    const int32_t *h_set;           // host copy of set.index (host class plan), else NULL
     const double *x0, *end_heading;
     double spacing;
     int collision_check, max_out;
@@ -744,7 +854,7 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     PQP_CUDA(cudaMemsetAsync(c.qp_states, 0, c.total * sizeof(pqp_state), st));   // stations past a cut read as zeros
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[1], st));
     // (1) bounds; n_valid = unblocked prefix of every path
-    int rc = launch_bounds_kernel(h, e, c.bounds_mode, c.batch, c.max_n, c.paths, c.map_index, c.bounds, st);
+    int rc = launch_bounds_kernel(h, e, c.bounds_mode, c.batch, c.max_n, c.paths, c.map_index, c.set, c.bounds, st);
     if (rc != PQP_OK) return rc;
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[2], st));
     // (2) QP on the unblocked prefix, every path on the kernel class of its own (length, keep_control_steps), exactly
@@ -760,7 +870,11 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
             PQP_CUDA(cudaMalloc(&h->d_max_k, (size_t)h->max_total * sizeof(double)));
             PQP_CUDA(cudaMalloc(&h->d_max_kp, (size_t)h->max_total * sizeof(double)));
         }
-        rc = pqp_update_limits_device(h, 0, (int)c.total, c.paths.ref, h->d_max_k, h->d_max_kp, st);
+        if (c.set.index)
+            rc = launch_limits_sets(h, c.batch, c.max_n, c.paths.n_points, c.paths.offsets, c.paths.ref, c.set, h->d_max_k,
+                                    h->d_max_kp, st);
+        else
+            rc = pqp_update_limits_device(h, 0, (int)c.total, c.paths.ref, h->d_max_k, h->d_max_kp, st);
         if (rc != PQP_OK) return rc;
         bv.max_k = h->d_max_k; bv.max_kp = h->d_max_kp;
     }
@@ -768,26 +882,23 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
         std::vector<int32_t> nv((size_t)c.batch);
         PQP_CUDA(cudaMemcpyAsync(nv.data(), e->d_nvalid, (size_t)c.batch * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         PQP_CUDA(cudaStreamSynchronize(st));
-        rc = pqp_launch_kp_classes(h, bv, c.batch, nv.data(), h->h_off, h_ref, nullptr, st, qp_launches, c.formulation);
+        rc = pqp_launch_kp_classes(h, bv, c.batch, nv.data(), h->h_off, h_ref, nullptr, st, qp_launches, c.formulation,
+                                   c.h_set);
     } else {
-        rc = pqp_launch_dispatch(h, bv, c.formulation, c.batch, (int)c.total, c.max_n, 0, 0, st, qp_launches);
+        rc = pqp_launch_dispatch(h, bv, c.formulation, c.batch, (int)c.total, c.max_n, 0, 0, st, qp_launches, c.set.index,
+                                 c.set.n_sets);
     }
     if (rc != PQP_OK) return rc;
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[3], st));
     // (3) tail
     if (c.output_mode == PQP_OUTPUT_RAW) {
-        TailArgs a;
-        a.maps = map_table(e, c.map_index); a.car = pqp::make_car_circles(h->params);
-        a.n_points = e->d_nvalid; a.offsets = c.paths.offsets; a.status = c.status; a.paths = c.qp_states;
-        a.collision_check = c.collision_check ? 1 : 0;
-        a.n_kept = c.out_n; a.ok = c.out_ok;
-        pqp_finish_raw_kernel<<<c.batch, 128, 0, st>>>(a);
-        PQP_CUDA(cudaGetLastError());
+        rc = launch_finish_raw(h, e, c.batch, e->d_nvalid, c.paths.offsets, c.status, c.map_index, c.set, c.qp_states,
+                               c.collision_check, c.out_n, c.out_ok, st);
     } else {
-        rc = launch_densify(h, e, c.batch, e->d_nvalid, c.paths.offsets, c.status, c.map_index, c.qp_states, c.spacing,
-                            c.collision_check, c.max_out, c.dense, c.out_n, c.out_ok, st);
-        if (rc != PQP_OK) return rc;
+        rc = launch_densify(h, e, c.batch, e->d_nvalid, c.paths.offsets, c.status, c.map_index, c.set, c.qp_states,
+                            c.spacing, c.collision_check, c.max_out, c.dense, c.out_n, c.out_ok, st);
     }
+    if (rc != PQP_OK) return rc;
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[4], st));
     return PQP_OK;
 }
@@ -798,15 +909,26 @@ int pqp_plan_batch_maps(pqp_handle *h, int formulation, int bounds_mode, int out
                         const double *x0, const double *end_heading, double output_spacing, int collision_check,
                         int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok, int32_t *status,
                         int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
+    return pqp_plan_batch_sets(h, formulation, bounds_mode, output_mode, batch, n_points, ref, map_index, nullptr, n_knots,
+                               knots, x_coef, y_coef, x0, end_heading, output_spacing, collision_check, max_out,
+                               out_states, out_n, out_ok, status, iters, out_bounds, stats);
+}
+
+int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                        const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                        const int32_t *param_index, const int32_t *n_knots, const double *knots, const double *x_coef,
+                        const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
+                        int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
+                        int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
     if (!h || batch < 0 || (batch > 0 && (!n_points || !ref || !x0 || !end_heading || !out_states || !out_n || !out_ok)) ||
         (bounds_mode != PQP_BOUNDS_IMPROVED && bounds_mode != PQP_BOUNDS_SIMPLE) ||
         (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
         (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch(_maps): bad argument");
+        pqp_set_err("pqp_plan_batch(_maps, _sets): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch(_maps): unknown formulation");
+        pqp_set_err("pqp_plan_batch(_maps, _sets): unknown formulation");
         return PQP_ERR_ARG;
     }
     if (stats) memset(stats, 0, sizeof(*stats));
@@ -829,6 +951,10 @@ int pqp_plan_batch_maps(pqp_handle *h, int formulation, int bounds_mode, int out
         PQP_CUDA(cudaMemcpyAsync(e->d_mapidx, map_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
         h2d += (int64_t)(B * sizeof(int32_t));
     }
+    if (param_index) {
+        PQP_CUDA(cudaMemcpyAsync(e->d_setidx, param_index, B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        h2d += (int64_t)(B * sizeof(int32_t));
+    }
     if (output_mode == PQP_OUTPUT_DENSIFY) {
         rc = grow(&e->d_dense, &e->dense_cap, B * (size_t)max_out * sizeof(pqp_state));
         if (rc != PQP_OK) return rc;
@@ -836,6 +962,8 @@ int pqp_plan_batch_maps(pqp_handle *h, int formulation, int bounds_mode, int out
     ChainIO c;
     c.formulation = formulation; c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
     c.max_n = max_n; c.total = T; c.paths = handle_paths(h, e); c.map_index = map_index ? e->d_mapidx : nullptr;
+    c.set = param_index ? SetIndex{e->d_setidx, (int)h->sets.size()} : kSet0;
+    c.h_set = param_index;
     c.x0 = h->d_x0; c.end_heading = h->d_end;
     c.spacing = output_spacing; c.collision_check = collision_check; c.max_out = max_out;
     c.qp_states = h->d_out; c.dense = e->d_dense; c.out_n = e->d_nkept; c.out_ok = e->d_ok;
@@ -904,18 +1032,32 @@ int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, 
                                int collision_check, int max_out, pqp_state *d_out_states, int32_t *d_out_n,
                                int32_t *d_out_ok, int32_t *d_status, int32_t *d_iters,
                                pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
-    if (!h || batch < 0 || total_points < 0 ||
+    return pqp_plan_batch_device_sets(h, formulation, bounds_mode, output_mode, batch, total_points, max_n_points, 0,
+                                      d_n_points, d_offsets, d_ref, d_map_index, nullptr, d_knot_offsets, d_knots,
+                                      d_x_coef, d_y_coef, d_x0, d_end_heading, output_spacing, collision_check, max_out,
+                                      d_out_states, d_out_n, d_out_ok, d_status, d_iters, d_out_bounds, stream, stats);
+}
+
+int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                               int total_points, int max_n_points, int n_param_sets, const int32_t *d_n_points,
+                               const int32_t *d_offsets, const pqp_state *d_ref, const int32_t *d_map_index,
+                               const int32_t *d_param_index, const int32_t *d_knot_offsets, const double *d_knots,
+                               const double *d_x_coef, const double *d_y_coef, const double *d_x0,
+                               const double *d_end_heading, double output_spacing, int collision_check, int max_out,
+                               pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok, int32_t *d_status,
+                               int32_t *d_iters, pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
+    if (!h || batch < 0 || total_points < 0 || n_param_sets < 0 ||
         (batch > 0 && (!d_n_points || !d_offsets || !d_ref || !d_x0 || !d_end_heading || !d_out_states || !d_out_n ||
                        !d_out_ok || !d_status)) ||
         (bounds_mode != PQP_BOUNDS_IMPROVED && bounds_mode != PQP_BOUNDS_SIMPLE) ||
         (bounds_mode == PQP_BOUNDS_IMPROVED && batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef)) ||
         (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
         (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch_device(_maps): bad argument");
+        pqp_set_err("pqp_plan_batch_device(_maps, _sets): bad argument");
         return PQP_ERR_ARG;
     }
     if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch_device(_maps): unknown formulation");
+        pqp_set_err("pqp_plan_batch_device(_maps, _sets): unknown formulation");
         return PQP_ERR_ARG;
     }
     if (stats) memset(stats, 0, sizeof(*stats));
@@ -935,6 +1077,9 @@ int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, 
     c.total = (size_t)total_points;
     c.paths = PathsView{d_n_points, d_offsets, d_ref, d_knot_offsets, d_knots, d_x_coef, d_y_coef};
     c.map_index = d_map_index;
+    const int n_sets = (int)h->sets.size();
+    c.set = d_param_index ? SetIndex{d_param_index, n_param_sets > 0 ? std::min(n_param_sets, n_sets) : n_sets} : kSet0;
+    c.h_set = nullptr;
     c.x0 = d_x0; c.end_heading = d_end_heading;
     c.spacing = output_spacing; c.collision_check = collision_check; c.max_out = max_out;
     c.qp_states = output_mode == PQP_OUTPUT_RAW ? d_out_states : h->d_out;

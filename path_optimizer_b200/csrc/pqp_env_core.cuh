@@ -289,6 +289,41 @@ inline CarCircles make_car_circles(const pqp_params &p) {
     return c;
 }
 
+// What the stages either side of the QP read of one parameter set (pqp_set_param_sets): the covering-circle radius and
+// offsets d1..d4 of the bounds, the footprint of the collision check and the "KPC" limits (mu, curvature rate, and
+// kmax = tan(max_steering_angle) / wheel_base for limits rebuilt from splines).
+struct ParamRow {
+    double radius, d[4];
+    CarCircles car;
+    double mu, rate, kmax;
+};
+
+inline ParamRow make_param_row(const pqp_params &p) {
+    ParamRow r;
+    r.radius = p.circle_radius;
+    r.d[0] = p.d1; r.d[1] = p.d2; r.d[2] = p.d3; r.d[3] = p.d4;
+    r.car = make_car_circles(p);
+    r.mu = p.mu; r.rate = p.max_curvature_rate;
+    r.kmax = tan(p.max_steering_angle) / p.wheel_base;
+    return r;
+}
+
+// The parameter sets of a handle as the kernels see them, passed by value, so that a captured launch keeps the sets it
+// was captured with (as the solve kernels keep their by-value pqp::DevParams): R rows of which the first n are in use,
+// and an optional per-path index into them (NULL: row 0 for every path).  R = 1 without an index, PQP_MAX_PARAM_SETS
+// with one.
+template <int R> struct ParamTable {
+    ParamRow row[R];
+    int n;
+    const int32_t *index;
+};
+
+// Path b's row, or NULL when its index lies outside [0, n): the index is checked before the rows are read.
+template <int R> PQP_HD const ParamRow *param_of(const ParamTable<R> &t, int b) {
+    const int k = t.index ? t.index[b] : 0;
+    return (k >= 0 && k < t.n) ? &t.row[k] : nullptr;
+}
+
 // isSingleStateCollisionFreeImproved (:41-59) -> isSingleStateCollisionFree (:17-39)
 PQP_HD bool state_collision_free(const MapView &m, const CarCircles &c, double sx, double sy, double sz) {
     const double cz = cos(sz), sn = sin(sz);

@@ -19,9 +19,12 @@ struct pqp_handle {
     int max_batch = 0, max_total = 0;
     int smem_optin = 0;
     int num_sms = 0;
-    pqp_params params;
+    pqp_params params;               // set 0
     pqp::DevParams dprm;
     pqp::DevParams dprm_gen[2];
+    // the parameter sets (pqp_set_param_sets); params / dprm above are set 0
+    std::vector<pqp_params> sets;
+    std::vector<pqp::DevParams> dsets;
     cudaStream_t stream = nullptr;
     cudaStream_t stream2 = nullptr;                 // second lane of the host-buffer pipeline
     cudaEvent_t ev_chunk[PQP_MAX_CHUNKS + 2] = {};  // [0] shared arrays uploaded, [1+k] chunk k kernels done, [last] lane 2 drained
@@ -38,13 +41,15 @@ struct pqp_handle {
     int dc_nmax = -1, dc_klo = -1, dc_khi = -1, dc_skip = -1, dc_v = -1, dc_form = 0;
     size_t dc_smem = 0;
     // class plan of the last pqp_launch_kp_classes call (reused while the batch shape stays the same)
+    // launch segment g = set * (classes) + class; the entries past the last segment name the paths whose set index is
+    // out of range (n_reject of them)
     struct ClassPlan {
         bool valid = false;
-        int skip = 0, form = 0;
+        int skip = 0, form = 0, n_sets = 1, n_reject = 0;
         cudaStream_t stream = nullptr;
-        std::vector<int32_t> n, keep;
-        int count_v[PQP_MAX_VARIANTS] = {}, start_v[PQP_MAX_VARIANTS + 1] = {};
-        size_t smem_v[PQP_MAX_VARIANTS] = {};
+        std::vector<int32_t> n, keep, set;   // (set: empty without a set index)
+        std::vector<int> count, start;
+        std::vector<size_t> smem;
     } plan;
     // pqp_set_order_hint: expected ADMM iterations per path (e.g. the previous planning cycle's counts); launch order
     // inside a class becomes longest-expected-first
@@ -57,6 +62,12 @@ struct pqp_handle {
     int cls_ncols[3] = {}, cls_off[3] = {};
     int32_t *d_disp_order = nullptr, *d_disp_key = nullptr;
     int32_t *d_disp_n = nullptr, *d_disp_status = nullptr, *d_disp_iters = nullptr;
+    // device dispatch over parameter sets: per-(set, class) order segments (set_cap x max classes x max_batch) and the
+    // (set, class, length) histogram in global memory (it outgrows shared memory), grow-only.  An outgrown pair stays
+    // allocated until pqp_destroy: a graph captured before the growth still reads it.
+    int32_t *d_set_order = nullptr, *d_set_hist = nullptr;
+    int set_cap = 0;
+    std::vector<void *> retired;
     // launches of the last bounds the dispatch was asked for (form, max_n, min_keep, max_keep as passed)
     struct DispatchLaunches {
         bool valid = false;
@@ -87,16 +98,22 @@ struct pqp_handle {
 // device-side counts (BatchView::n_points) must equal n.  keep[b] = keep_control_steps per path, or NULL to derive
 // them from the host copy `ref` of the reference states.  Used by pqp_plan_batch after the bounds stage and by
 // pqp_solve_batch_device_classes.
+// `set` [batch]: parameter set of every path (host), NULL: set 0.  A path whose set lies outside the handle's sets is not
+// launched: a small kernel reports it PQP_INVALID_PROBLEM (0 iterations, NaN states).
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
-                          const pqp_state *ref, const int32_t *keep, cudaStream_t st, int *launches, int form = 0 /* PQP_FORM_KP; 2 = KPC (bv.max_k / max_kp set) */);
+                          const pqp_state *ref, const int32_t *keep, cudaStream_t st, int *launches, int form = 0 /* PQP_FORM_KP; 2 = KPC (bv.max_k / max_kp set) */,
+                          const int32_t *set = nullptr);
 
 // Internal (pqp_capi.cu): the same launches when the station counts exist on the device only.  A dispatch kernel reads
 // them, derives keep_control_steps from the device-side reference states, looks every path up in the class table and
 // sorts the paths into per-class order segments (longest first); every class the bounds can reach is launched over its
 // segment.  A path outside the bounds (max_n, min_keep..max_keep; 0 = unknown) reports PQP_INVALID_PROBLEM.
 // `total` = offsets[batch] bounds the grid of each class.  No host synchronisation, no allocation.
+// `d_set` [batch] (device): parameter set of every path, NULL: set 0; with it every (set < n_sets, class) pair the bounds
+// reach is launched, n_sets = min(n_param_sets, the handle's count) (n_param_sets 0: the handle's count).  A path whose set
+// lies outside [0, n_sets) reports PQP_INVALID_PROBLEM.
 int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
-                        int max_keep, cudaStream_t st, int *launches);
+                        int max_keep, cudaStream_t st, int *launches, const int32_t *d_set = nullptr, int n_param_sets = 0);
 
 // thread-local error text returned by pqp_last_error()
 extern thread_local char pqp_g_err[512];

@@ -159,11 +159,14 @@ class PathPlanner(BatchPathSolver):
         return dict(states=out, n_out=n_out, ok=ok, stats=stats)
 
     def plan(self, batch, formulation="KP", bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW,
-             output_spacing=0.3, collision_check=True, max_out=512, want_bounds=False, out=None, map_index=None):
+             output_spacing=0.3, collision_check=True, max_out=512, want_bounds=False, out=None, map_index=None,
+             param_index=None):
         """PathOptimizer::solveWithoutSmoothing for every path of the batch (bounds -> QP -> tail).
         `out` may carry a preallocated (e.g. pinned) `states` array of the output shape.  `map_index`: int32 [B], the
         map of the set (set_maps) every path is planned on (pqp_plan_batch_maps); None: map 0 (pqp_plan_batch).  A path
-        whose index is outside the set reports status -100 (invalid problem), 0 iterations, n_out = 0 and ok = 0."""
+        whose index is outside the set reports status -100 (invalid problem), 0 iterations, n_out = 0 and ok = 0.
+        `param_index`: int32 [B], the parameter set (set_param_sets) every path is planned with (pqp_plan_batch_sets);
+        None: set 0.  An index outside the sets fails its path the same way."""
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
         B = len(n_points)
@@ -187,13 +190,18 @@ class PathPlanner(BatchPathSolver):
         tail = (ptr(nk), ptr(kn), ptr(xc), ptr(yc), ptr(x0), ptr(end_heading), float(output_spacing),
                 int(collision_check), int(max_out), ptr(states), ptr(n_out), ptr(ok), ptr(status), ptr(iters),
                 ptr(bounds), C.byref(stats))
-        if map_index is None:
-            name, rc = "pqp_plan_batch", self._L.pqp_plan_batch(*head, *tail)
-        else:
+        mi = None
+        if map_index is not None:
             mi = np.asarray(map_index)
             if mi.shape != (B,) or mi.dtype.kind not in "iu":
                 raise ValueError(f"map_index: expected an integer array of shape ({B},), got {mi.dtype} {mi.shape}")
             mi = np.ascontiguousarray(mi, dtype=np.int32)
+        if param_index is not None:
+            pi = self._param_index(param_index, B)
+            name, rc = "pqp_plan_batch_sets", self._L.pqp_plan_batch_sets(*head, ptr(mi), ptr(pi), *tail)
+        elif map_index is None:
+            name, rc = "pqp_plan_batch", self._L.pqp_plan_batch(*head, *tail)
+        else:
             name, rc = "pqp_plan_batch_maps", self._L.pqp_plan_batch_maps(*head, ptr(mi), *tail)
         if rc != OK:
             raise PqpError(f"{name} failed (rc={rc}): {_lib.last_error()}")
@@ -202,7 +210,8 @@ class PathPlanner(BatchPathSolver):
 
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
-                    collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None):
+                    collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None,
+                    param_index=None, n_param_sets=0):
         """plan() on torch CUDA tensors of the planner's device (path_optimizer_b200.device): n_points int32 [B],
         offsets int32 [B + 1], ref float64 [T, 7], x0 float64 [B, 3], end_heading float64 [B]; `splines` (IMPROVED)
         a dict of knot_offsets int32 [B + 1], knots [K], x_coef / y_coef [K, 4] (device.splines_to_device).  The whole
@@ -211,7 +220,10 @@ class PathPlanner(BatchPathSolver):
         max_n_points >= every n_points (0: the longest path any kernel class takes).  `out` may carry the output
         tensors (states: [T, 7] RAW or [B, max_out, 7] DENSIFY; n_out, ok, status, iters; bounds [T, 8]).
         `map_index`: int32 [B] on the device, the map of the set every path is planned on (pqp_plan_batch_device_maps,
-        as plan(map_index=...)); None: map 0.  A graph replay reads the index from the captured tensor."""
+        as plan(map_index=...)); None: map 0.  A graph replay reads the index from the captured tensor.
+        `param_index`: int32 [B] on the device, the parameter set of every path (pqp_plan_batch_device_sets, as
+        plan(param_index=...)); None: set 0.  n_param_sets > 0 bounds the sets launched (an index at or past it fails
+        its path).  A graph replays with the sets it was captured with."""
         import torch
         from . import device as D
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
@@ -241,7 +253,12 @@ class PathPlanner(BatchPathSolver):
         head = (self._h, form, int(bounds_mode), int(output_mode), B, T, int(max_n_points))
         tail = (float(output_spacing), int(collision_check), int(max_out), *outs,
                 torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
-        if map_index is None:
+        if param_index is not None:
+            mi = D.check(map_index, "map_index", i32, (B,), dev)
+            pi = D.check(param_index, "param_index", i32, (B,), dev)
+            name = "pqp_plan_batch_device_sets"
+            rc = self._L.pqp_plan_batch_device_sets(*head, int(n_param_sets), *args[:3], mi, pi, *args[3:], *tail)
+        elif map_index is None:
             name, rc = "pqp_plan_batch_device", self._L.pqp_plan_batch_device(*head, *args, *tail)
         else:
             mi = D.check(map_index, "map_index", i32, (B,), dev)

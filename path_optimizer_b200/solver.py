@@ -65,13 +65,34 @@ class BatchPathSolver:
         self.params = params
         self._L.pqp_set_params(self._h, C.byref(params))
 
+    def set_param_sets(self, sets):
+        """Replace the parameter sets (pqp_set_param_sets): a sequence of 1..64 Params, each already run through
+        pqp_params_update_config.  solve(), solve_device() and the planner's plan calls pick a path's set with
+        `param_index`; set 0 is what the calls without an index use.  A bad argument leaves the previous sets in place."""
+        sets = list(sets)
+        arr = (Params * max(len(sets), 1))(*sets)
+        rc = self._L.pqp_set_param_sets(self._h, len(sets), arr)
+        if rc != OK:
+            raise PqpError(f"pqp_set_param_sets failed (rc={rc}): {_lib.last_error()}")
+        self.params = sets[0]
+        self.param_sets = sets
+
+    @staticmethod
+    def _param_index(param_index, B):
+        pi = np.asarray(param_index)
+        if pi.shape != (B,) or pi.dtype.kind not in "iu":
+            raise ValueError(f"param_index: expected an integer array of shape ({B},), got {pi.dtype} {pi.shape}")
+        return np.ascontiguousarray(pi, dtype=np.int32)
+
     def max_points(self, formulation="KP"):
         return self._L.pqp_max_points(self._h, FORMULATIONS[formulation])
 
-    def solve(self, batch, formulation="KP", want_frenet=True, out=None, max_k=None, max_kp=None):
+    def solve(self, batch, formulation="KP", want_frenet=True, out=None, max_k=None, max_kp=None, param_index=None):
         """batch: dict as produced by synth.* (host numpy arrays).  Returns dict(states, frenet,
         status, iters, ok, stats).  `out` may carry preallocated (e.g. pinned) output arrays.
-        max_k / max_kp ([sum N] each) are the KPC limits (ReferencePath::getMaxKList / getMaxKpList)."""
+        max_k / max_kp ([sum N] each) are the KPC limits (ReferencePath::getMaxKList / getMaxKpList).
+        `param_index`: int32 [B], the parameter set (set_param_sets) every path is solved with (pqp_solve_batch_sets);
+        None: set 0.  A path whose index is outside the sets reports status -100 with 0 iterations and NaN states."""
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
         B = len(n_points)
@@ -91,11 +112,15 @@ class BatchPathSolver:
             max_k = np.ascontiguousarray(max_k, dtype=np.float64)
             max_kp = np.ascontiguousarray(max_kp, dtype=np.float64)
             assert len(max_k) == total and len(max_kp) == total
-        rc = self._L.pqp_solve_batch(self._h, form, B, ptr(n_points), ptr(ref), ptr(bounds), ptr(x0),
-                                     ptr(end_heading), ptr(max_k), ptr(max_kp), ptr(states), ptr(frenet), ptr(status),
-                                     ptr(iters), C.byref(stats))
+        head = (self._h, form, B, ptr(n_points), ptr(ref), ptr(bounds), ptr(x0), ptr(end_heading), ptr(max_k), ptr(max_kp))
+        tail = (ptr(states), ptr(frenet), ptr(status), ptr(iters), C.byref(stats))
+        if param_index is None:
+            name, rc = "pqp_solve_batch", self._L.pqp_solve_batch(*head, *tail)
+        else:
+            pi = self._param_index(param_index, B)
+            name, rc = "pqp_solve_batch_sets", self._L.pqp_solve_batch_sets(*head, ptr(pi), *tail)
         if rc != OK:
-            raise PqpError(f"pqp_solve_batch failed (rc={rc}): {_lib.last_error()}")
+            raise PqpError(f"{name} failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, frenet=frenet, status=status, iters=iters, ok=(status == SOLVED), stats=stats)
 
     def _cuda_device(self):
@@ -103,14 +128,17 @@ class BatchPathSolver:
         return torch.device("cuda", int(self.device))
 
     def solve_device(self, n_points, offsets, ref, bounds, x0, end_heading, formulation="KP", max_n_points=0,
-                     min_keep=0, max_keep=0, max_k=None, max_kp=None, want_frenet=True, out=None, stats=False):
+                     min_keep=0, max_keep=0, max_k=None, max_kp=None, want_frenet=True, out=None, stats=False,
+                     param_index=None, n_param_sets=0):
         """The batch as torch CUDA tensors on the solver's device (path_optimizer_b200.device): n_points int32 [B],
         offsets int32 [B + 1], ref float64 [T, 7], bounds float64 [T, 8], x0 float64 [B, 3], end_heading float64 [B],
         KPC limits float64 [T].  Every path runs on the kernel class solve() would choose for it, picked on the device
         (pqp_solve_batch_device_dispatch), with solve()'s results bit for bit.  Runs on torch.cuda.current_stream()
         without synchronising it (unless `stats`), so that after one warm-up call it can be captured in a CUDA graph.
         max_n_points / min_keep / max_keep (0 = unknown) only narrow the classes launched; a path outside them reports
-        INVALID_PROBLEM.  `out` may carry the output tensors (states, frenet, status, iters).  Returns them as a dict."""
+        INVALID_PROBLEM.  `out` may carry the output tensors (states, frenet, status, iters).  Returns them as a dict.
+        `param_index`: int32 [B] on the device, the parameter set of every path (pqp_solve_batch_device_dispatch_sets);
+        None: set 0.  n_param_sets > 0 bounds the sets launched (an index at or past it reports INVALID_PROBLEM)."""
         import torch
         from . import device as D
         form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
@@ -132,11 +160,17 @@ class BatchPathSolver:
                 D.check(states, "states", f64, (T, D.STATE_COLS), dev), D.check(frenet, "frenet", f64, (T, 3), dev),
                 D.check(status, "status", i32, (B,), dev), D.check(iters, "iters", i32, (B,), dev)]
         st = Stats()
-        rc = self._L.pqp_solve_batch_device_dispatch(self._h, form, B, T, int(max_n_points), int(min_keep), int(max_keep),
-                                                     *args, torch.cuda.current_stream(dev).cuda_stream,
-                                                     C.byref(st) if stats else None)
+        tail = (torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
+        bounds_ = (self._h, form, B, T, int(max_n_points), int(min_keep), int(max_keep))
+        if param_index is None:
+            name = "pqp_solve_batch_device_dispatch"
+            rc = self._L.pqp_solve_batch_device_dispatch(*bounds_, *args, *tail)
+        else:
+            pi = D.check(param_index, "param_index", i32, (B,), dev)
+            name = "pqp_solve_batch_device_dispatch_sets"
+            rc = self._L.pqp_solve_batch_device_dispatch_sets(*bounds_, int(n_param_sets), *args[:8], pi, *args[8:], *tail)
         if rc != OK:
-            raise PqpError(f"pqp_solve_batch_device_dispatch failed (rc={rc}): {_lib.last_error()}")
+            raise PqpError(f"{name} failed (rc={rc}): {_lib.last_error()}")
         return dict(states=states, frenet=frenet, status=status, iters=iters, stats=st if stats else None)
 
 

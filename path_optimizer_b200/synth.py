@@ -304,3 +304,56 @@ def multi_map_batch(n_maps, n_candidates, n=200, seed=BASE_SEED, first_maps=(), 
     elif order != "grouped":
         raise ValueError(f"order: 'grouped' or 'interleaved', got {order!r}")
     return maps, b, np.ascontiguousarray(map_index, dtype=np.int32)
+
+
+# ---------------------------------------------------------------------------------------------
+# Many parameter sets in one batch (pqp_set_param_sets + a set index per path)
+# ---------------------------------------------------------------------------------------------
+
+def param_sets(k, seed=BASE_SEED):
+    """k valid parameter sets (Params, run through pqp_params_update_config) for one batch.  Set 0 is the reference's
+    defaults.  The others cycle through five variants, each with seeded jitter, so that any five consecutive sets from 1
+    on differ in every group the stages read:
+      1: vehicle geometry (car width / length, safety margin: radius and d1..d4), wheel base and steering limit, the
+         "KPC" limits (mu, curvature rate);
+      2: the weights (a nonzero KP_deviation_weight, KP and K weights), expected_safety_margin, constraint_end_heading = 0;
+      3: OSQP tolerances an order of magnitude tighter and adaptive_rho_interval = 100;
+      4: max_iter = 50 (most paths end PQP_MAX_ITER_REACHED) with another geometry and KPC limits;
+      5: mild jitter of geometry and weights only."""
+    import ctypes as C
+
+    from . import _lib
+    from .solver import default_params
+    rng = np.random.default_rng(seed)
+    L = _lib.load()
+    out = []
+    for s in range(k):
+        p = default_params()
+        if s > 0:
+            v = (s - 1) % 5 + 1
+            j = lambda lo, hi: float(rng.uniform(lo, hi))   # noqa: E731
+            if v == 1:
+                p.car_width, p.car_length, p.safety_margin = 1.8 + j(-0.05, 0.05), 4.5 + j(-0.1, 0.1), 0.1 + j(0, 0.05)
+                p.wheel_base, p.max_steering_angle = 2.6 + j(-0.05, 0.05), np.deg2rad(35.0 + j(-2, 2))
+                p.mu, p.max_curvature_rate = 0.6 + j(-0.05, 0.05), 0.15 + j(-0.01, 0.01)
+            elif v == 2:
+                p.KP_deviation_weight, p.KP_curvature_weight = 5.0 + j(0, 2), 20.0 + j(-2, 2)
+                p.KP_curvature_rate_weight, p.KP_slack_weight = 150.0 + j(-10, 10), 4.0 + j(0, 1)
+                p.K_curvature_weight, p.K_curvature_rate_weight = 30.0 + j(-3, 3), 300.0 + j(-20, 20)
+                p.K_deviation_weight = 2.0 + j(0, 1)
+                p.expected_safety_margin = 1.0 + j(-0.05, 0.05)
+                p.constraint_end_heading = 0
+            elif v == 3:
+                p.eps_abs = p.eps_rel = 1e-4 * (1.0 + j(0, 0.5))
+                p.eps_prim_inf = p.eps_dual_inf = 1e-5
+                p.adaptive_rho_interval = 100
+            elif v == 4:
+                p.max_iter = 50
+                p.car_width, p.car_length, p.safety_margin = 2.2 + j(-0.05, 0.05), 5.2 + j(-0.1, 0.1), 0.2
+                p.mu, p.max_curvature_rate = 0.3 + j(-0.02, 0.02), 0.05 + j(0, 0.01)
+            else:
+                p.car_width, p.car_length = 2.0 + j(-0.1, 0.1), 4.9 + j(-0.2, 0.2)
+                p.KP_curvature_weight, p.K_curvature_weight = 10.0 + j(-2, 2), 50.0 + j(-5, 5)
+        L.pqp_params_update_config(C.byref(p))
+        out.append(p)
+    return out
