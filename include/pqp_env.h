@@ -68,6 +68,49 @@ int pqp_set_map(pqp_handle *h, const pqp_distance_map *map);
  * is no reference counterpart for several maps. */
 int pqp_set_maps(pqp_handle *h, int n_maps, const pqp_distance_map *maps);
 
+/* An occupancy grid from which the device builds a distance layer: the `binary` matrix the reference passes to
+ * cv::distanceTransform.  `cells` is ROW-major [rows][cols] in the index convention of pqp_distance_map; a cell value of
+ * 0 is an obstacle, any other value is free.  Geometry as pqp_distance_map. */
+typedef struct pqp_occupancy_map {
+    const uint8_t *cells;
+    int32_t rows, cols;
+    double resolution;
+    double center_x, center_y;
+} pqp_occupancy_map;
+
+/* Replace the handle's map set with `n_maps` >= 1 layers built on the device from occupancy grids, as pqp_set_maps
+ * replaces it from finished layers: every descriptor is checked first (NULL cells, rows or cols < 1, resolution <= 0:
+ * PQP_ERR_ARG, the previous set stays), the layers go into the same grow-only cell buffer and table, and afterwards every
+ * entry sees an ordinary map set.  Only the uint8 cells are uploaded (a quarter of the bytes of a layer).  Synchronous.
+ * Layer of a map: the exact Euclidean distance transform.  With d2 the squared distance, in cells, from a cell's centre
+ * to the nearest obstacle cell's centre (64-bit integers), the cell holds (float)sqrt((double)d2) * (float)resolution,
+ * one float multiply; obstacle cells hold 0, and cells outside the grid are not obstacles.  That is bit for bit
+ * ndimage.distance_transform_edt(cells != 0).astype(float32) * float32(resolution), and within 1 ulp of
+ * cv::distanceTransform(CV_DIST_L2, CV_DIST_MASK_PRECISE) * resolution.  A grid with no obstacle gets OpenCV's value on
+ * every cell: 2^64 * resolution.
+ * Replaces: cv::distanceTransform(binary, CV_DIST_L2, CV_DIST_MASK_PRECISE) * resolution and Map(grid_map) per scene
+ * (path_optimizer_benchmark.cpp:28-43, demo.cpp:103-110). */
+int pqp_set_maps_occupancy(pqp_handle *h, int n_maps, const pqp_occupancy_map *maps);
+
+/* pqp_set_maps_occupancy with DEVICE `cells` pointers (a host array of descriptors), asynchronous on `stream` (NULL: the
+ * handle's stream).
+ *   Same layout: when n_maps and every map's rows, cols, resolution and centre equal the handle's current set, and an
+ *   earlier occupancy call has sized the transform's scratch for that set, the call only launches the transform (two
+ *   kernels per 256 maps): no allocation, no copy, no host synchronisation.  It can then be captured in a CUDA graph
+ *   together with pqp_plan_batch_device(_maps, _sets).
+ *   Otherwise it lays the set out anew and synchronises.  If `stream` is capturing it returns PQP_ERR_ARG instead, before
+ *   it touches the stream, so the capture stays valid.
+ *   Replay: a replayed build writes map m only if table row m still has the cell address, rows and cols it was captured
+ *   with; otherwise that map's build does nothing.  A replay after a later layout change leaves the current set as it
+ *   is, and a plan in the same graph reads the current set (the table-growth rule of pqp_set_maps applies).
+ * No reference counterpart: the reference builds its layer on the host. */
+int pqp_set_maps_occupancy_device(pqp_handle *h, int n_maps, const pqp_occupancy_map *maps, void *stream);
+
+/* Copy map m's layer (rows * cols floats, row-major) of the handle's set into the host buffer `out`, synchronously on
+ * the handle's stream (synchronise the stream of a pqp_set_maps_occupancy_device call first).  PQP_ERR_ARG when m is
+ * outside [0, n_maps) or `out` is NULL.  No reference counterpart (grid_map's layer is host memory there). */
+int pqp_get_map(pqp_handle *h, int m, float *out);
+
 /* Map::getObstacleDistance (Map.cpp:16-22) for `n` positions xy[n][2] on the device: bilinear
  * interpolation of the four surrounding cell centres, nearest cell when a neighbour falls outside
  * the grid, 0 outside the map; result rounded to float like grid_map's atPosition.  Map 0 of the

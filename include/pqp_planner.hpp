@@ -15,6 +15,7 @@
 #ifndef PQP_PLANNER_HPP_
 #define PQP_PLANNER_HPP_
 
+#include <utility>
 #include <vector>
 
 #include "pqp_env.h"
@@ -28,6 +29,15 @@ struct DistanceMap {
     int rows = 0, cols = 0;
     double resolution = 0, center_x = 0, center_y = 0;
     pqp_distance_map view() const { return pqp_distance_map{distance.data(), rows, cols, resolution, center_x, center_y}; }
+};
+
+// Row-major occupancy grid, 0 = obstacle: the `binary` matrix the reference passes to cv::distanceTransform before it
+// wraps the result in a grid_map (path_optimizer_benchmark.cpp:28-43).  Same index convention as DistanceMap.
+struct OccupancyMap {
+    std::vector<uint8_t> cells;
+    int rows = 0, cols = 0;
+    double resolution = 0, center_x = 0, center_y = 0;
+    pqp_occupancy_map view() const { return pqp_occupancy_map{cells.data(), rows, cols, resolution, center_x, center_y}; }
 };
 
 // tk::spline's interface (natural boundary, quadratic extrapolation): set_points, operator(), deriv.
@@ -80,7 +90,43 @@ class PathOptimizerGpu {
             std::fprintf(stderr, "pqp_set_maps failed: %s\n", pqp_last_error());
             return nullptr;
         }
+        for (const DistanceMap &m : maps) p->shapes_.push_back({m.rows, m.cols});
         return p;
+    }
+
+    // The same from occupancy grids: the layers are built on the device (pqp_set_maps_occupancy), in place of
+    // cv::distanceTransform(binary, CV_DIST_L2, CV_DIST_MASK_PRECISE) * resolution on the host.
+    static std::unique_ptr<PathOptimizerGpu> create(const std::vector<OccupancyMap> &maps, int max_batch,
+                                                    int max_total_points, const pqp_params *params = nullptr,
+                                                    int device = 0) {
+        std::unique_ptr<PathOptimizerGpu> p(new PathOptimizerGpu);
+        if (!p->handle_.open(params, device, max_batch, max_total_points)) {
+            std::fprintf(stderr, "pqp_create failed: %s\n", pqp_last_error());
+            return nullptr;
+        }
+        if (!p->setMaps(maps)) return nullptr;
+        return p;
+    }
+
+    // Replace the maps with layers built on the device from occupancy grids (the next scene of a sweep, moved
+    // obstacles).  On failure the previous maps stay.
+    bool setMaps(const std::vector<OccupancyMap> &maps) {
+        std::vector<pqp_occupancy_map> v;
+        for (const OccupancyMap &m : maps) v.push_back(m.view());
+        if (pqp_set_maps_occupancy(handle_.get(), (int)v.size(), v.data()) != PQP_OK) {
+            std::fprintf(stderr, "pqp_set_maps_occupancy failed: %s\n", pqp_last_error());
+            return false;
+        }
+        shapes_.clear();
+        for (const OccupancyMap &m : maps) shapes_.push_back({m.rows, m.cols});
+        return true;
+    }
+
+    // The distance layer of map m (rows * cols floats, row-major), e.g. to show what the paths were planned against.
+    bool getMap(int m, std::vector<float> *layer) const {
+        if (!layer || m < 0 || m >= (int)shapes_.size()) return false;
+        layer->resize((size_t)shapes_[m].first * shapes_[m].second);
+        return pqp_get_map(handle_.get(), m, layer->data()) == PQP_OK;
     }
 
     // Several parameter sets as well (pqp_set_param_sets): param_sets[k] is set k of the batched solveWithoutSmoothing's
@@ -252,6 +298,7 @@ class PathOptimizerGpu {
     }
     PathOptimizerGpu() = default;
     Handle handle_;
+    std::vector<std::pair<int, int>> shapes_;   // rows, cols of every map
 };
 
 }  // namespace pqp

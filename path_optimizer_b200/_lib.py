@@ -3,7 +3,7 @@ product has no CPU fallback."""
 import ctypes as C
 import os
 
-from .abi import DistanceMap, Params, Stats
+from .abi import DistanceMap, OccupancyMap, Params, Stats
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PQP_LIB") or os.path.join(_HERE, "libpqp.so")   # PQP_LIB: A/B builds of the same ABI
@@ -19,7 +19,7 @@ SYMBOLS = ["pqp_params_default", "pqp_params_update_config", "pqp_keep_control_s
 ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "pqp_map_distance", "pqp_spline_fit", "pqp_spline_eval", "pqp_update_bounds_batch",
                "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device",
                "pqp_set_maps", "pqp_plan_batch_maps", "pqp_plan_batch_device_maps", "pqp_plan_batch_sets",
-               "pqp_plan_batch_device_sets"]
+               "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -91,6 +91,9 @@ def load():
                                       [C.c_double, C.c_int, C.c_int] + [vp] * 6 + [C.POINTER(Stats)])
     L.pqp_plan_batch_device_sets.argtypes = ([vp] + [C.c_int] * 7 + [vp] * 11 + [C.c_double, C.c_int, C.c_int] +
                                              [vp] * 7 + [C.POINTER(Stats)])
+    L.pqp_set_maps_occupancy.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap)]
+    L.pqp_set_maps_occupancy_device.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap), vp]
+    L.pqp_get_map.argtypes = [vp, C.c_int, vp]
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

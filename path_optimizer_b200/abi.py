@@ -73,6 +73,12 @@ class DistanceMap(C.Structure):
                 ("resolution", C.c_double), ("center_x", C.c_double), ("center_y", C.c_double)]
 
 
+class OccupancyMap(C.Structure):
+    """``pqp_occupancy_map`` (include/pqp_env.h)."""
+    _fields_ = [("cells", C.c_void_p), ("rows", C.c_int32), ("cols", C.c_int32),
+                ("resolution", C.c_double), ("center_x", C.c_double), ("center_y", C.c_double)]
+
+
 def ptr(arr, ctype=C.c_void_p):
     """Raw pointer of a C-contiguous numpy array (or None)."""
     if arr is None:

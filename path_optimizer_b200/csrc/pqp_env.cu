@@ -14,6 +14,7 @@
 #include <new>
 #include <vector>
 
+#include "pqp_edt_core.cuh"
 #include "pqp_env_core.cuh"
 #include "pqp_handle.h"
 
@@ -35,6 +36,14 @@ struct EnvState {
     size_t maps_cap = 0;
     int32_t *d_nmaps = nullptr;
     int n_maps = 0;                // 0: no map set
+    std::vector<MapView> h_maps;   // host copy of the table (n_maps rows)
+    // occupancy builds (pqp_set_maps_occupancy*): the uploaded cells of the host entry, and the transform's scratch
+    // (3 int32 per cell, at three times a map's cell offset).  An outgrown scratch goes to the handle's retired list: a
+    // graph captured before still writes it.
+    uint8_t *d_occ = nullptr;
+    size_t occ_cap = 0;
+    int32_t *d_edt = nullptr;
+    size_t edt_cap = 0;
     // per-batch scratch (sized from the handle's capacity at first use)
     int32_t *d_nvalid = nullptr, *d_nkept = nullptr, *d_ok = nullptr, *d_koff = nullptr;
     int32_t *d_mapidx = nullptr;   // pqp_plan_batch_maps: the uploaded map index
@@ -56,7 +65,7 @@ void env_free(void *p) {
     cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx); cudaFree(e->d_setidx);
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
-    cudaFree(e->d_tmp);
+    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     delete e;
 }
@@ -309,9 +318,143 @@ pqp_densify_kernel(const __grid_constant__ DensifyArgs<R> a) {
     }
 }
 
+// Occupancy builds (pqp_edt_core.cuh): one launch per pass covers up to kEdtMaps maps, blockIdx.y = map of the launch.
+// The builds are passed by value, so a captured launch keeps the occupancy and destination it was captured with; before
+// it writes anything a map's threads check that table row `index` still describes that destination (address, rows,
+// cols), so a replay after a later layout change leaves the current set alone.
+constexpr int kEdtMaps = 256;
+struct EdtMap {
+    const uint8_t *occ;      // [rows][cols], 0 = obstacle
+    float *dst;              // the layer's cells in the map buffer
+    int32_t *scratch;        // 3 * rows * cols
+    int rows, cols;
+    float res;
+    int index;               // row of the table
+};
+struct EdtArgs {
+    const MapView *table;
+    const int32_t *n_maps;
+    EdtMap map[kEdtMaps];
+};
+static_assert(sizeof(EdtArgs) <= 32764, "the build descriptors must fit a kernel's parameter space");
+
+__device__ __forceinline__ bool edt_current(const EdtArgs &a, const EdtMap &m) {
+    if (m.index >= *a.n_maps) return false;
+    const MapView &v = a.table[m.index];
+    return v.d == m.dst && v.rows == m.rows && v.cols == m.cols;
+}
+
+// grid (ceil(max cols / 128), maps): thread = column
+__global__ void __launch_bounds__(128)
+pqp_edt_column_kernel(const __grid_constant__ EdtArgs a) {
+    const EdtMap &m = a.map[blockIdx.y];
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m.cols || !edt_current(a, m)) return;
+    pqp::edt_column(m.occ, m.rows, m.cols, j, m.scratch + (size_t)j * m.rows, 1);
+}
+
+// grid (ceil(max rows / 128), maps): thread = row
+__global__ void __launch_bounds__(128)
+pqp_edt_row_kernel(const __grid_constant__ EdtArgs a) {
+    const EdtMap &m = a.map[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m.rows || !edt_current(a, m)) return;
+    const size_t R = (size_t)m.rows, n = R * (size_t)m.cols;
+    pqp::edt_row(m.scratch + i, R, m.cols, m.scratch + n + i, m.scratch + 2 * n + i, R, m.res,
+                 m.dst + (size_t)i * m.cols);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host helpers
 // ---------------------------------------------------------------------------------------------
+
+// Lays out a set of n_maps geometries (each map's cells start on a 256-byte boundary of the one cell buffer): grows the
+// cell buffer and the table, and writes the table and the count on `st`.  The caller fills the cells, synchronises and
+// then publishes the set (e->n_maps, e->h_maps); until then the handle has none.  `Desc`: pqp_distance_map or
+// pqp_occupancy_map.
+template <typename Desc>
+int lay_out_maps(EnvState *e, int n_maps, const Desc *maps, cudaStream_t st, std::vector<MapView> *table) {
+    constexpr size_t kAlign = 256 / sizeof(float);
+    std::vector<size_t> first((size_t)n_maps);
+    size_t cells = 0;
+    for (int m = 0; m < n_maps; ++m) {
+        first[m] = cells;
+        cells += ((size_t)maps[m].rows * (size_t)maps[m].cols + kAlign - 1) / kAlign * kAlign;
+    }
+    e->n_maps = 0;   // no set until the new one is in place
+    e->h_maps.clear();
+    int rc = grow(&e->d_map, &e->map_cap, cells * sizeof(float));
+    if (rc != PQP_OK) return rc;
+    rc = grow(&e->d_maps, &e->maps_cap, (size_t)n_maps * sizeof(MapView));
+    if (rc != PQP_OK) return rc;
+    table->resize((size_t)n_maps);
+    for (int m = 0; m < n_maps; ++m) {
+        const Desc &d = maps[m];
+        (*table)[m] = pqp::make_map_view(e->d_map + first[m], d.rows, d.cols, d.resolution, d.center_x, d.center_y);
+    }
+    const int32_t count = n_maps;
+    PQP_CUDA(cudaMemcpyAsync(e->d_maps, table->data(), table->size() * sizeof(MapView), cudaMemcpyHostToDevice, st));
+    PQP_CUDA(cudaMemcpyAsync(e->d_nmaps, &count, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    return PQP_OK;
+}
+
+// Bytes of transform scratch a table needs: 3 int32 per cell of the map buffer up to the end of its last map.
+size_t edt_need(const EnvState *e, const std::vector<MapView> &table) {
+    size_t end = 0;
+    for (const MapView &v : table) end = std::max(end, (size_t)(v.d - e->d_map) + (size_t)v.rows * v.cols);
+    return 3 * end * sizeof(int32_t);
+}
+
+// Launches the build of every map of `table` from the occupancy grids occ[m] (device pointers).
+int launch_edt(EnvState *e, const std::vector<MapView> &table, const uint8_t *const *occ, cudaStream_t st) {
+    const int n_maps = (int)table.size();
+    for (int first = 0; first < n_maps; first += kEdtMaps) {
+        EdtArgs a;
+        a.table = e->d_maps;
+        a.n_maps = e->d_nmaps;
+        const int n = std::min(kEdtMaps, n_maps - first);
+        int max_rows = 0, max_cols = 0;
+        for (int k = 0; k < n; ++k) {
+            const MapView &v = table[first + k];
+            const size_t off = (size_t)(v.d - e->d_map);
+            a.map[k] = EdtMap{occ[first + k], const_cast<float *>(v.d), e->d_edt + 3 * off, v.rows, v.cols, (float)v.res,
+                              first + k};
+            max_rows = std::max(max_rows, v.rows);
+            max_cols = std::max(max_cols, v.cols);
+        }
+        pqp_edt_column_kernel<<<dim3((unsigned)((max_cols + 127) / 128), (unsigned)n), 128, 0, st>>>(a);
+        PQP_CUDA(cudaGetLastError());
+        pqp_edt_row_kernel<<<dim3((unsigned)((max_rows + 127) / 128), (unsigned)n), 128, 0, st>>>(a);
+        PQP_CUDA(cudaGetLastError());
+    }
+    return PQP_OK;
+}
+
+// Checks occupancy descriptors as pqp_set_maps checks its own.
+bool occupancy_ok(int n_maps, const pqp_occupancy_map *maps) {
+    if (n_maps < 1 || !maps) return false;
+    for (int m = 0; m < n_maps; ++m) {
+        const pqp_occupancy_map &d = maps[m];
+        if (!d.cells || d.rows < 1 || d.cols < 1 || !(d.resolution > 0.0)) return false;
+    }
+    return true;
+}
+
+// Lays out an occupancy set and sizes the transform's scratch (an outgrown one is retired, not freed).
+int lay_out_occupancy(pqp_handle *h, EnvState *e, int n_maps, const pqp_occupancy_map *maps, cudaStream_t st,
+                      std::vector<MapView> *table) {
+    int rc = lay_out_maps(e, n_maps, maps, st, table);
+    if (rc != PQP_OK) return rc;
+    const size_t need = edt_need(e, *table);
+    if (need > e->edt_cap) {
+        if (e->d_edt) h->retired.push_back(e->d_edt);
+        e->d_edt = nullptr;
+        e->edt_cap = 0;
+        PQP_CUDA(cudaMalloc(&e->d_edt, need));
+        e->edt_cap = need;
+    }
+    return PQP_OK;
+}
 
 int need_map(pqp_handle *h, EnvState **e) {
     int rc = env_get(h, e);
@@ -483,35 +626,108 @@ int pqp_set_maps(pqp_handle *h, int n_maps, const pqp_distance_map *maps) {
     int rc = env_get(h, &e);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaSetDevice(h->device));
-    // each map starts on a 256-byte boundary of the one cell buffer
-    constexpr size_t kAlign = 256 / sizeof(float);
-    std::vector<size_t> first((size_t)n_maps);
-    size_t cells = 0;
-    for (int m = 0; m < n_maps; ++m) {
-        first[m] = cells;
-        cells += ((size_t)maps[m].rows * (size_t)maps[m].cols + kAlign - 1) / kAlign * kAlign;
-    }
-    e->n_maps = 0;   // no set until the new one is in place
-    rc = grow(&e->d_map, &e->map_cap, cells * sizeof(float));
+    std::vector<MapView> table;
+    rc = lay_out_maps(e, n_maps, maps, h->stream, &table);
     if (rc != PQP_OK) return rc;
-    rc = grow(&e->d_maps, &e->maps_cap, (size_t)n_maps * sizeof(MapView));
-    if (rc != PQP_OK) return rc;
-    std::vector<MapView> table((size_t)n_maps);
     for (int m = 0; m < n_maps; ++m) {
         const pqp_distance_map &d = maps[m];
-        float *dst = e->d_map + first[m];
-        PQP_CUDA(cudaMemcpyAsync(dst, d.distance, (size_t)d.rows * d.cols * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-        table[m] = pqp::make_map_view(dst, d.rows, d.cols, d.resolution, d.center_x, d.center_y);
+        PQP_CUDA(cudaMemcpyAsync(const_cast<float *>(table[m].d), d.distance, (size_t)d.rows * d.cols * sizeof(float),
+                                 cudaMemcpyHostToDevice, h->stream));
     }
-    const int32_t count = n_maps;
-    PQP_CUDA(cudaMemcpyAsync(e->d_maps, table.data(), table.size() * sizeof(MapView), cudaMemcpyHostToDevice, h->stream));
-    PQP_CUDA(cudaMemcpyAsync(e->d_nmaps, &count, sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
     PQP_CUDA(cudaStreamSynchronize(h->stream));
     e->n_maps = n_maps;
+    e->h_maps.swap(table);
     return PQP_OK;
 }
 
 int pqp_set_map(pqp_handle *h, const pqp_distance_map *map) { return pqp_set_maps(h, 1, map); }
+
+int pqp_set_maps_occupancy(pqp_handle *h, int n_maps, const pqp_occupancy_map *maps) {
+    // every descriptor is checked before any device state changes: a bad one leaves the previous set in place
+    if (!h || !occupancy_ok(n_maps, maps)) {
+        pqp_set_err("pqp_set_maps_occupancy: bad argument (needs a handle and n_maps >= 1 descriptors with cells, rows "
+                    "and cols >= 1 and resolution > 0)");
+        return PQP_ERR_ARG;
+    }
+    EnvState *e;
+    int rc = env_get(h, &e);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    std::vector<MapView> table;
+    rc = lay_out_occupancy(h, e, n_maps, maps, st, &table);
+    if (rc != PQP_OK) return rc;
+    // the cells go to the upload buffer at the maps' cell offsets
+    const MapView &last = table.back();
+    rc = grow(&e->d_occ, &e->occ_cap, (size_t)(last.d - e->d_map) + (size_t)last.rows * last.cols);
+    if (rc != PQP_OK) return rc;
+    std::vector<const uint8_t *> occ((size_t)n_maps);
+    for (int m = 0; m < n_maps; ++m) {
+        uint8_t *dst = e->d_occ + (table[m].d - e->d_map);
+        PQP_CUDA(cudaMemcpyAsync(dst, maps[m].cells, (size_t)maps[m].rows * maps[m].cols, cudaMemcpyHostToDevice, st));
+        occ[m] = dst;
+    }
+    rc = launch_edt(e, table, occ.data(), st);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaStreamSynchronize(st));
+    e->n_maps = n_maps;
+    e->h_maps.swap(table);
+    return PQP_OK;
+}
+
+int pqp_set_maps_occupancy_device(pqp_handle *h, int n_maps, const pqp_occupancy_map *maps, void *stream) {
+    if (!h || !occupancy_ok(n_maps, maps)) {
+        pqp_set_err("pqp_set_maps_occupancy_device: bad argument (needs a handle and n_maps >= 1 descriptors with cells, "
+                    "rows and cols >= 1 and resolution > 0)");
+        return PQP_ERR_ARG;
+    }
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    std::vector<const uint8_t *> occ((size_t)n_maps);
+    for (int m = 0; m < n_maps; ++m) occ[m] = maps[m].cells;
+    EnvState *e = (EnvState *)h->env;
+    bool same = e && e->n_maps == n_maps && (int)e->h_maps.size() == n_maps;
+    for (int m = 0; same && m < n_maps; ++m) {
+        const MapView &v = e->h_maps[m];
+        const pqp_occupancy_map &d = maps[m];
+        same = v.rows == d.rows && v.cols == d.cols && v.res == d.resolution && v.cx == d.center_x && v.cy == d.center_y;
+    }
+    if (same && edt_need(e, e->h_maps) <= e->edt_cap) {
+        PQP_CUDA(cudaSetDevice(h->device));
+        return launch_edt(e, e->h_maps, occ.data(), st);
+    }
+    // a new layout allocates and synchronises, which a capture must not see
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    PQP_CUDA(cudaStreamIsCapturing(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone) {
+        pqp_set_err("pqp_set_maps_occupancy_device: the map layout changes (count, rows, cols, resolution or centre), "
+                    "which cannot be captured; make one call with this layout before capturing");
+        return PQP_ERR_ARG;
+    }
+    int rc = env_get(h, &e);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    std::vector<MapView> table;
+    rc = lay_out_occupancy(h, e, n_maps, maps, st, &table);
+    if (rc != PQP_OK) return rc;
+    rc = launch_edt(e, table, occ.data(), st);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaStreamSynchronize(st));
+    e->n_maps = n_maps;
+    e->h_maps.swap(table);
+    return PQP_OK;
+}
+
+int pqp_get_map(pqp_handle *h, int m, float *out) {
+    if (!h || !out || m < 0 || !h->env || m >= ((EnvState *)h->env)->n_maps) {
+        pqp_set_err("pqp_get_map: bad argument (needs a handle, an output buffer and a map of the set)");
+        return PQP_ERR_ARG;
+    }
+    const MapView &v = ((EnvState *)h->env)->h_maps[m];
+    PQP_CUDA(cudaSetDevice(h->device));
+    PQP_CUDA(cudaMemcpyAsync(out, v.d, (size_t)v.rows * v.cols * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    PQP_CUDA(cudaStreamSynchronize(h->stream));
+    return PQP_OK;
+}
 
 int pqp_map_distance(pqp_handle *h, int n, const double *xy, double *out) {
     if (!h || n < 0 || (n > 0 && (!xy || !out))) { pqp_set_err("pqp_map_distance: bad argument"); return PQP_ERR_ARG; }

@@ -16,7 +16,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .abi import (BOUNDS_DTYPE, FORMULATIONS, OK, SOLVED, STATE_DTYPE, DistanceMap, Stats, ptr)
+from .abi import (BOUNDS_DTYPE, FORMULATIONS, OK, SOLVED, STATE_DTYPE, DistanceMap, OccupancyMap, Stats, ptr)
 from .solver import BatchPathSolver, PqpError
 
 BOUNDS_IMPROVED, BOUNDS_SIMPLE = 0, 1
@@ -78,6 +78,7 @@ class PathPlanner(BatchPathSolver):
         rc = self._L.pqp_set_map(self._h, C.byref(dm))
         if rc != OK:
             raise PqpError(f"pqp_set_map failed (rc={rc}): {_lib.last_error()}")
+        self._map_shapes = [dist.shape]
 
     def set_maps(self, maps):
         """Replace the map set with several maps (pqp_set_maps), each a dict in the form set_map takes; plan() and
@@ -92,6 +93,61 @@ class PathPlanner(BatchPathSolver):
         rc = self._L.pqp_set_maps(self._h, len(maps), dms)
         if rc != OK:
             raise PqpError(f"pqp_set_maps failed (rc={rc}): {_lib.last_error()}")
+        self._map_shapes = [d.shape for d in dists]
+
+    @staticmethod
+    def _occupancy_descriptors(maps, cells):
+        oms = (OccupancyMap * max(len(maps), 1))()
+        for i, (m, (p, rows, cols)) in enumerate(zip(maps, cells)):
+            oms[i] = OccupancyMap(p, rows, cols, float(m["resolution"]), float(m["center_x"]), float(m["center_y"]))
+        return oms
+
+    def set_maps_occupancy(self, maps):
+        """Replace the map set with layers the device builds from occupancy grids (pqp_set_maps_occupancy): each map a
+        dict of `occupancy` uint8 [rows, cols] (0 = obstacle, anything else free), resolution, center_x, center_y.  A
+        layer is the exact Euclidean distance transform in metres, bit for bit
+        ndimage.distance_transform_edt(occupancy != 0).astype(float32) * float32(resolution) (synth.distance_layer)."""
+        maps = list(maps)
+        occ = [np.ascontiguousarray(m["occupancy"], dtype=np.uint8) for m in maps]
+        if any(o.ndim != 2 for o in occ):
+            raise ValueError("occupancy: expected uint8 arrays of shape [rows, cols]")
+        oms = self._occupancy_descriptors(maps, [(o.ctypes.data, o.shape[0], o.shape[1]) for o in occ])
+        rc = self._L.pqp_set_maps_occupancy(self._h, len(maps), oms)
+        if rc != OK:
+            raise PqpError(f"pqp_set_maps_occupancy failed (rc={rc}): {_lib.last_error()}")
+        self._map_shapes = [o.shape for o in occ]
+
+    def set_maps_occupancy_device(self, maps):
+        """set_maps_occupancy with `occupancy` as torch uint8 CUDA tensors [rows, cols] on the planner's device
+        (pqp_set_maps_occupancy_device), on torch.cuda.current_stream().  With the geometry of the current set (after
+        one such call) it only launches the transform and can be captured in a CUDA graph with plan_device; a new layout
+        synchronises and is refused while the stream is capturing."""
+        import torch
+        from . import device as D
+        dev = self._cuda_device()
+        maps = list(maps)
+        cells = []
+        for m in maps:
+            t = m["occupancy"]
+            shape = tuple(t.shape) if isinstance(t, torch.Tensor) else ()
+            if len(shape) != 2:
+                raise ValueError("occupancy: expected uint8 CUDA tensors of shape [rows, cols]")
+            cells.append((D.check(t, "occupancy", torch.uint8, shape, dev), shape[0], shape[1]))
+        oms = self._occupancy_descriptors(maps, cells)
+        rc = self._L.pqp_set_maps_occupancy_device(self._h, len(maps), oms, torch.cuda.current_stream(dev).cuda_stream)
+        if rc != OK:
+            raise PqpError(f"pqp_set_maps_occupancy_device failed (rc={rc}): {_lib.last_error()}")
+        self._map_shapes = [(rows, cols) for _, rows, cols in cells]
+
+    def get_map(self, m):
+        """Layer of map m of the set (pqp_get_map): float32 [rows, cols].  Synchronise the stream of a
+        set_maps_occupancy_device call first."""
+        shapes = getattr(self, "_map_shapes", [])
+        out = np.empty(shapes[m] if 0 <= m < len(shapes) else (0, 0), dtype=np.float32)
+        rc = self._L.pqp_get_map(self._h, int(m), ptr(out))
+        if rc != OK:
+            raise PqpError(f"pqp_get_map failed (rc={rc}): {_lib.last_error()}")
+        return out
 
     def map_distance(self, xy):
         xy = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)

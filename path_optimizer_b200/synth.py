@@ -172,16 +172,35 @@ def slice_batch(batch, begin, end):
 # Config 3: obstacle field + distance map (the input of the clearance-bounds stage)
 # ---------------------------------------------------------------------------------------------
 
+def distance_layer(occupancy, resolution):
+    """The distance layer of an occupancy grid (0 = obstacle): exact Euclidean distance transform in metres, float32,
+    ndimage.distance_transform_edt(occupancy != 0).astype(float32) * float32(resolution).  Within 1 ulp of what the
+    reference builds with cv::distanceTransform(L2, MASK_PRECISE) * resolution (path_optimizer_benchmark.cpp:39-43), and
+    bit for bit what PathPlanner.set_maps_occupancy builds on the device (except on a grid with no obstacle, where the
+    device writes OpenCV's 2^64 * resolution)."""
+    from scipy import ndimage
+    dist = ndimage.distance_transform_edt(np.asarray(occupancy) != 0).astype(np.float32) * np.float32(resolution)
+    return np.ascontiguousarray(dist)
+
+
 def disc_field_map(rows=1100, cols=250, resolution=0.2, n_discs=300, seed=BASE_SEED, config=3,
                    center=(0.0, 0.0), keep_clear_halfwidth=1.7):
-    """Synthetic 0.2 m occupancy grid with random discs (radius U(0.5, 2) m) and its Euclidean
-    distance transform in metres -- what the reference builds with cv::distanceTransform(L2,
-    MASK_PRECISE) * resolution (path_optimizer_benchmark.cpp:39-43).  Discs whose edge would come
-    within `keep_clear_halfwidth` of the map's x axis are pushed out so that a corridor exists.
+    """disc_field_occupancy and its distance layer (distance_layer) -- what the reference builds with
+    cv::distanceTransform(L2, MASK_PRECISE) * resolution (path_optimizer_benchmark.cpp:39-43).  Returns dict(distance
+    float32 [rows, cols], rows, cols, resolution, center_x, center_y)."""
+    occ = disc_field_occupancy(rows, cols, resolution, n_discs, seed, config, center, keep_clear_halfwidth)
+    return dict(distance=distance_layer(occ["occupancy"], resolution), rows=rows, cols=cols,
+                resolution=float(resolution), center_x=float(center[0]), center_y=float(center[1]))
+
+
+def disc_field_occupancy(rows=1100, cols=250, resolution=0.2, n_discs=300, seed=BASE_SEED, config=3,
+                         center=(0.0, 0.0), keep_clear_halfwidth=1.7):
+    """Synthetic 0.2 m occupancy grid with random discs (radius U(0.5, 2) m), 0 inside a disc and 1 elsewhere: the
+    `binary` matrix the reference passes to cv::distanceTransform.  Discs whose edge would come within
+    `keep_clear_halfwidth` of the map's x axis are pushed out so that a corridor exists.
     grid_map index convention: cell (i, j) centred at x = cx + L_x/2 - (i+0.5) res,
-    y = cy + L_y/2 - (j+0.5) res.  Returns dict(distance float32 [rows, cols], rows, cols,
-    resolution, center_x, center_y)."""
-    from scipy import ndimage
+    y = cy + L_y/2 - (j+0.5) res.  Returns dict(occupancy uint8 [rows, cols], rows, cols, resolution, center_x,
+    center_y): the form PathPlanner.set_maps_occupancy takes."""
     lx, ly = rows * resolution, cols * resolution
     xs = center[0] + lx / 2 - (np.arange(rows) + 0.5) * resolution
     ys = center[1] + ly / 2 - (np.arange(cols) + 0.5) * resolution
@@ -196,8 +215,7 @@ def disc_field_map(rows=1100, cols=250, resolution=0.2, n_discs=300, seed=BASE_S
         if gap < keep_clear_halfwidth:
             y0 = center[1] + np.sign(y0 - center[1] if y0 != center[1] else 1.0) * (keep_clear_halfwidth + rad[k])
         free &= ((xs[:, None] - cx[k]) ** 2 + (ys[None, :] - y0) ** 2) > rad[k] ** 2
-    dist = ndimage.distance_transform_edt(free).astype(np.float32) * np.float32(resolution)
-    return dict(distance=np.ascontiguousarray(dist), rows=rows, cols=cols, resolution=float(resolution),
+    return dict(occupancy=free.astype(np.uint8), rows=rows, cols=cols, resolution=float(resolution),
                 center_x=float(center[0]), center_y=float(center[1]))
 
 
