@@ -364,6 +364,62 @@ int pqp_solve_batch_device_dispatch_sets(pqp_handle *h, int formulation, int bat
                                          void *stream,
                                          pqp_stats *stats);
 
+/* pqp_solve_batch_sets and pqp_solve_batch_device_dispatch_sets with one formulation per path in place of the scalar:
+ * `formulation` (host) or `d_formulation` (device), int32 [batch] of PQP_FORM_* values, so that one call can mix
+ * "KP", "K" and "KPC" paths (e.g. vehicles configured for "KPC" beside vehicles on "KP", or the three formulations of
+ * the same scenes side by side).  The array is required.
+ *   Path b's results -- status, iterations, states and Frenet states -- equal, bit for bit, those the _sets entry gives
+ *   it when called with formulation = formulation[b], for any mix of parameter sets and lengths in the batch.
+ *   A formulation outside {0, 1, 2}, or for the device entry outside `form_mask`, makes only that path report
+ *   PQP_INVALID_PROBLEM (0 iterations, NaN states); no other path changes.  Set indices keep their rules.
+ *   form_mask      device entry: bitmask of 1 << PQP_FORM_*, 0 = all three.  Like n_param_sets it only bounds what is
+ *                  launched: one grid per reachable (set, kernel class) pair of the formulations in the mask.
+ *   max_n_points   device entry: as for the _sets entry, for every formulation (0: unknown); each path stays limited
+ *                  by its own formulation's classes ("KPC" 256 stations, "KP" 408 at keep 3..4, "K" 416).
+ *   max_k, max_kp  the "KPC" limits: PQP_ERR_ARG when NULL and some path is "KPC" (host entry) or the mask holds
+ *                  "KPC" (device entry).  "KP" and "K" paths do not read them.
+ * The host entry plans one launch segment per (set, kernel class), with each path on the class of its own formulation.
+ * The device entry keeps every promise of pqp_solve_batch_device_dispatch_sets: asynchronous on `stream`, no host
+ * synchronisation unless `stats` is non-NULL, no allocation after a warm-up call with the same or a larger mask and set
+ * count, capturable in a CUDA graph (a replay reads the formulations from the captured array).  Its sort needs device
+ * scratch of its own.  With PQP_GENERIC_K / PQP_GENERIC_KPC set and a path of that formulation, the host entry
+ * returns PQP_ERR_UNSUPPORTED.
+ * Replaces: OsqpSolver::create(FLAGS_optimization_method, ...) + solve (solver.cpp:30-77) once per path, with that
+ * path's FLAGS_optimization_method. */
+int pqp_solve_batch_forms(pqp_handle *h, int batch,
+                          const int32_t *n_points,
+                          const pqp_state *ref,
+                          const pqp_station_bounds *bounds,
+                          const double *x0,
+                          const double *end_heading,
+                          const double *max_k,
+                          const double *max_kp,
+                          const int32_t *param_index,
+                          const int32_t *formulation,
+                          pqp_state *out_states,
+                          double *out_frenet,
+                          int32_t *status,
+                          int32_t *iters,
+                          pqp_stats *stats);
+int pqp_solve_batch_device_dispatch_forms(pqp_handle *h, int batch, int total_points,
+                                          int max_n_points, int min_keep, int max_keep, int n_param_sets,
+                                          int form_mask,
+                                          const int32_t *d_n_points, const int32_t *d_offsets,
+                                          const pqp_state *d_ref,
+                                          const pqp_station_bounds *d_bounds,
+                                          const double *d_x0,
+                                          const double *d_end_heading,
+                                          const double *d_max_k,
+                                          const double *d_max_kp,
+                                          const int32_t *d_param_index,
+                                          const int32_t *d_formulation,
+                                          pqp_state *d_out_states,
+                                          double *d_out_frenet,
+                                          int32_t *d_status,
+                                          int32_t *d_iters,
+                                          void *stream,
+                                          pqp_stats *stats);
+
 /* Last error text for this thread (CUDA error strings etc.); never NULL. */
 /* Launch-order hint for the next solves of a batch of `batch` paths: expected ADMM iterations per path, e.g. the
  * `iters` the previous planning cycle reported for the same candidates.  Inside a kernel class the paths are then

@@ -306,6 +306,49 @@ int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, 
                                int32_t *d_status, int32_t *d_iters,
                                pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats);
 
+/* pqp_plan_batch_sets and pqp_plan_batch_device_sets with one formulation per path in place of the scalar:
+ * `formulation` (host) or `d_formulation` (device), int32 [batch] of PQP_FORM_* values; the array is required.
+ *   Path b's results -- status, iterations, states, bounds, out_n and ok -- equal, bit for bit, those the _sets entry
+ *   gives it when called with formulation = formulation[b], for any mix of maps, sets and lengths in the batch.
+ *   A formulation outside {0, 1, 2}, or for the device entry outside `form_mask`, makes only that path report
+ *   PQP_INVALID_PROBLEM with 0 iterations, out_n = 0 and ok = 0; no other path changes.  Map and set indices keep
+ *   their rules.
+ *   form_mask      device entry: bitmask of 1 << PQP_FORM_*, 0 = all three; it only bounds what is launched.
+ *   max_n_points   device entry: 0 = the longest path any class of any formulation in the mask takes.  Each path stays
+ *                  limited by its own formulation's classes, as in its _sets call; a longer one reports
+ *                  PQP_INVALID_PROBLEM (its bounds past that limit are then computed, where the _sets call leaves them
+ *                  unwritten).
+ * The "KPC" limits are derived on the device, as the chain does for a "KPC" call, whenever some path is "KPC" (host
+ * entry) or the mask holds "KPC" (device entry); "KP" and "K" paths do not read them.  The bounds and tail stages do
+ * not depend on the formulation.  The device entry keeps every promise of pqp_plan_batch_device_sets (no allocation
+ * after a warm-up call with the same or a larger mask and set count; a CUDA graph replay reads the formulations from
+ * the captured array).
+ * Replaces: PathOptimizer::solveWithoutSmoothing (path_optimizer.cpp:87-117) once per path, with that path's
+ * FLAGS_optimization_method. */
+int pqp_plan_batch_forms(pqp_handle *h, int bounds_mode, int output_mode, int batch,
+                         const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                         const int32_t *param_index, const int32_t *formulation,
+                         const int32_t *n_knots, const double *knots,
+                         const double *x_coef, const double *y_coef,
+                         const double *x0, const double *end_heading,
+                         double output_spacing, int collision_check, int max_out,
+                         pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
+                         int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds,
+                         pqp_stats *stats);
+int pqp_plan_batch_device_forms(pqp_handle *h, int bounds_mode, int output_mode,
+                                int batch, int total_points, int max_n_points, int n_param_sets,
+                                int form_mask,
+                                const int32_t *d_n_points, const int32_t *d_offsets,
+                                const pqp_state *d_ref, const int32_t *d_map_index,
+                                const int32_t *d_param_index, const int32_t *d_formulation,
+                                const int32_t *d_knot_offsets, const double *d_knots,
+                                const double *d_x_coef, const double *d_y_coef,
+                                const double *d_x0, const double *d_end_heading,
+                                double output_spacing, int collision_check, int max_out,
+                                pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok,
+                                int32_t *d_status, int32_t *d_iters,
+                                pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats);
+
 #ifdef __cplusplus
 } /* extern "C" */
 #endif

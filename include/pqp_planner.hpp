@@ -15,6 +15,7 @@
 #ifndef PQP_PLANNER_HPP_
 #define PQP_PLANNER_HPP_
 
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -211,6 +212,25 @@ class PathOptimizerGpu {
                     ok, x_s, y_s, status);
     }
 
+    // The same with method[b] ("KP", "K" or "KPC") the FLAGS_optimization_method reference b is planned with as well
+    // (pqp_plan_batch_forms): PathOptimizer::solveWithoutSmoothing once per reference with that reference's
+    // FLAGS_optimization_method, the "KPC" limits derived from the v, a fields of its states as updateLimits does.  An
+    // empty map_index / param_index means map 0 / set 0 for every reference.  A reference whose method is no
+    // formulation gets ok = 0, an empty path and status PQP_INVALID_PROBLEM.
+    bool solveWithoutSmoothing(const std::vector<std::vector<State>> &references, const std::vector<VehicleStateView> &vehicle,
+                               const std::vector<int32_t> &map_index, const std::vector<int32_t> &param_index,
+                               const std::vector<std::string> &method, std::vector<std::vector<State>> *final_paths,
+                               std::vector<char> *ok, const std::vector<Spline> *x_s = nullptr,
+                               const std::vector<Spline> *y_s = nullptr, std::vector<int32_t> *status = nullptr) {
+        if ((!map_index.empty() && map_index.size() != references.size()) ||
+            (!param_index.empty() && param_index.size() != references.size()) || method.size() != references.size())
+            return false;
+        std::vector<int32_t> forms(method.size());
+        for (size_t b = 0; b < method.size(); ++b) forms[b] = formulation_from_type(method[b]);
+        return plan(references, vehicle, map_index.empty() ? nullptr : map_index.data(),
+                    param_index.empty() ? nullptr : param_index.data(), final_paths, ok, x_s, y_s, status, forms.data());
+    }
+
     // The reference's single-path signature (path_optimizer.cpp:87-88).
     bool solveWithoutSmoothing(const std::vector<State> &reference_points, const VehicleStateView &vehicle,
                                std::vector<State> *final_path) {
@@ -226,11 +246,12 @@ class PathOptimizerGpu {
 
  private:
     // Batched solveWithoutSmoothing (pqp_plan_batch_sets; map_index NULL: map 0, param_index NULL: set 0 for every
-    // reference).
+    // reference; forms non-NULL: pqp_plan_batch_forms with that formulation per reference).
     bool plan(const std::vector<std::vector<State>> &references, const std::vector<VehicleStateView> &vehicle,
               const int32_t *map_index, const int32_t *param_index, std::vector<std::vector<State>> *final_paths,
               std::vector<char> *ok,
-              const std::vector<Spline> *x_s, const std::vector<Spline> *y_s, std::vector<int32_t> *status) {
+              const std::vector<Spline> *x_s, const std::vector<Spline> *y_s, std::vector<int32_t> *status,
+              const int32_t *forms = nullptr) {
         const int B = (int)references.size();
         Packed in;
         if (!final_paths || !ok || (int)vehicle.size() < B || !pack(references, x_s, y_s, &in)) return false;
@@ -244,14 +265,21 @@ class PathOptimizerGpu {
         const bool raw = enable_raw_output;
         std::vector<State> out(raw ? in.ref.size() : (size_t)B * max_output_states);
         std::vector<int32_t> n_out(B), okv(B), st(B);
-        const int rc = pqp_plan_batch_sets(handle_.get(), PQP_FORM_KP, in.mode, raw ? PQP_OUTPUT_RAW : PQP_OUTPUT_DENSIFY,
-                                           B, in.n.data(), reinterpret_cast<const pqp_state *>(in.ref.data()), map_index,
-                                           param_index, in.nk_ptr(), in.knots_ptr(), in.xc_ptr(), in.yc_ptr(), x0.data(),
-                                           endh.data(), output_spacing, enable_collision_check ? 1 : 0, max_output_states,
-                                           reinterpret_cast<pqp_state *>(out.data()), n_out.data(), okv.data(), st.data(),
-                                           nullptr, nullptr, nullptr);
+        const int om = raw ? PQP_OUTPUT_RAW : PQP_OUTPUT_DENSIFY;
+        const pqp_state *ref = reinterpret_cast<const pqp_state *>(in.ref.data());
+        const int rc =
+            forms ? pqp_plan_batch_forms(handle_.get(), in.mode, om, B, in.n.data(), ref, map_index, param_index, forms,
+                                         in.nk_ptr(), in.knots_ptr(), in.xc_ptr(), in.yc_ptr(), x0.data(), endh.data(),
+                                         output_spacing, enable_collision_check ? 1 : 0, max_output_states,
+                                         reinterpret_cast<pqp_state *>(out.data()), n_out.data(), okv.data(), st.data(),
+                                         nullptr, nullptr, nullptr)
+                  : pqp_plan_batch_sets(handle_.get(), PQP_FORM_KP, in.mode, om, B, in.n.data(), ref, map_index,
+                                        param_index, in.nk_ptr(), in.knots_ptr(), in.xc_ptr(), in.yc_ptr(), x0.data(),
+                                        endh.data(), output_spacing, enable_collision_check ? 1 : 0, max_output_states,
+                                        reinterpret_cast<pqp_state *>(out.data()), n_out.data(), okv.data(), st.data(),
+                                        nullptr, nullptr, nullptr);
         if (rc != PQP_OK) {
-            std::fprintf(stderr, "pqp_plan_batch_sets failed: %s\n", pqp_last_error());
+            std::fprintf(stderr, "%s failed: %s\n", forms ? "pqp_plan_batch_forms" : "pqp_plan_batch_sets", pqp_last_error());
             return false;
         }
         final_paths->assign(B, {});

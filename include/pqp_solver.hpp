@@ -142,12 +142,31 @@ class BatchPathSolver {
         return solve(n_points, reference_states, bounds, vehicle, param_index.data(), out);
     }
 
+    // The same with method[b] ("KP", "K" or "KPC") the FLAGS_optimization_method path b is solved with
+    // (pqp_solve_batch_forms): OsqpSolver::create(method[b], ...) and solve once per path.  An empty param_index means
+    // set 0 for every path.  A path whose method is no formulation reports PQP_INVALID_PROBLEM, as the reference's
+    // create returns nullptr for it.  "KPC" paths read max_k / max_kp (concatenated like reference_states;
+    // ReferencePath::getMaxKList / getMaxKpList); without them a batch with a "KPC" path fails with PQP_ERR_ARG.
+    bool solve(const std::vector<int32_t> &n_points, const std::vector<State> &reference_states,
+               const std::vector<CoveringCircleBounds> &bounds, const std::vector<VehicleStateView> &vehicle,
+               const std::vector<int32_t> &param_index, const std::vector<std::string> &method, Result *out,
+               const std::vector<double> *max_k = nullptr, const std::vector<double> *max_kp = nullptr) {
+        if ((!param_index.empty() && param_index.size() != n_points.size()) || method.size() != n_points.size())
+            return false;
+        std::vector<int32_t> forms(method.size());
+        for (size_t b = 0; b < method.size(); ++b) forms[b] = formulation_from_type(method[b]);
+        return solve(n_points, reference_states, bounds, vehicle, param_index.empty() ? nullptr : param_index.data(), out,
+                     forms.data(), max_k ? max_k->data() : nullptr, max_kp ? max_kp->data() : nullptr);
+    }
+
     pqp_handle *handle() const { return handle_.get(); }
 
  private:
+    // forms NULL: pqp_solve_batch_sets with the solver's type; else pqp_solve_batch_forms
     bool solve(const std::vector<int32_t> &n_points, const std::vector<State> &reference_states,
                const std::vector<CoveringCircleBounds> &bounds, const std::vector<VehicleStateView> &vehicle,
-               const int32_t *param_index, Result *out) {
+               const int32_t *param_index, Result *out, const int32_t *forms = nullptr, const double *max_k = nullptr,
+               const double *max_kp = nullptr) {
         const int batch = (int)n_points.size();
         size_t total = 0;
         for (int n : n_points) total += (size_t)n;
@@ -163,13 +182,19 @@ class BatchPathSolver {
         out->frenet.assign(3 * total, 0.0);
         out->status.assign(batch, PQP_UNSOLVED);
         out->iters.assign(batch, 0);
-        out->rc = pqp_solve_batch_sets(handle_.get(), form_, batch, n_points.data(),
-                                       reinterpret_cast<const pqp_state *>(reference_states.data()),
-                                       reinterpret_cast<const pqp_station_bounds *>(bounds.data()), x0.data(),
-                                       endh.data(), nullptr, nullptr, param_index,
-                                       reinterpret_cast<pqp_state *>(out->states.data()), out->frenet.data(),
-                                       out->status.data(), out->iters.data(), &out->stats);
-        if (out->rc != PQP_OK) std::fprintf(stderr, "pqp_solve_batch_sets failed: %s\n", pqp_last_error());
+        const pqp_state *ref = reinterpret_cast<const pqp_state *>(reference_states.data());
+        const pqp_station_bounds *bnd = reinterpret_cast<const pqp_station_bounds *>(bounds.data());
+        pqp_state *states = reinterpret_cast<pqp_state *>(out->states.data());
+        if (forms)
+            out->rc = pqp_solve_batch_forms(handle_.get(), batch, n_points.data(), ref, bnd, x0.data(), endh.data(), max_k,
+                                            max_kp, param_index, forms, states, out->frenet.data(), out->status.data(),
+                                            out->iters.data(), &out->stats);
+        else
+            out->rc = pqp_solve_batch_sets(handle_.get(), form_, batch, n_points.data(), ref, bnd, x0.data(), endh.data(),
+                                           nullptr, nullptr, param_index, states, out->frenet.data(), out->status.data(),
+                                           out->iters.data(), &out->stats);
+        if (out->rc != PQP_OK)
+            std::fprintf(stderr, "%s failed: %s\n", forms ? "pqp_solve_batch_forms" : "pqp_solve_batch_sets", pqp_last_error());
         return out->rc == PQP_OK;
     }
 

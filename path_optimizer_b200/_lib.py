@@ -14,12 +14,13 @@ SYMBOLS = ["pqp_params_default", "pqp_params_update_config", "pqp_keep_control_s
            "pqp_solve_batch_device_classes", "pqp_last_error", "pqp_version", "pqp_max_points", "pqp_max_points_keep",
            "pqp_class_info", "pqp_class_info_kpc", "pqp_class_info_form", "pqp_set_order_hint", "pqp_class_name", "pqp_device_class_info",
            "pqp_solve_batch_device_dispatch", "pqp_class_table", "pqp_set_param_sets", "pqp_solve_batch_sets",
-           "pqp_solve_batch_device_dispatch_sets"]
+           "pqp_solve_batch_device_dispatch_sets", "pqp_solve_batch_forms", "pqp_solve_batch_device_dispatch_forms"]
 # ... and include/pqp_env.h
 ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "pqp_map_distance", "pqp_spline_fit", "pqp_spline_eval", "pqp_update_bounds_batch",
                "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device",
                "pqp_set_maps", "pqp_plan_batch_maps", "pqp_plan_batch_device_maps", "pqp_plan_batch_sets",
-               "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map"]
+               "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map",
+               "pqp_plan_batch_forms", "pqp_plan_batch_device_forms"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -66,6 +67,8 @@ def load():
     L.pqp_set_param_sets.argtypes = [vp, C.c_int, C.POINTER(Params)]
     L.pqp_solve_batch_sets.argtypes = [vp, C.c_int, C.c_int] + [vp] * 12 + [C.POINTER(Stats)]
     L.pqp_solve_batch_device_dispatch_sets.argtypes = [vp] + [C.c_int] * 7 + [vp] * 14 + [C.POINTER(Stats)]
+    L.pqp_solve_batch_forms.argtypes = [vp, C.c_int] + [vp] * 13 + [C.POINTER(Stats)]
+    L.pqp_solve_batch_device_dispatch_forms.argtypes = [vp] + [C.c_int] * 7 + [vp] * 15 + [C.POINTER(Stats)]
     # include/pqp_env.h
     L.pqp_update_limits.argtypes = [C.POINTER(Params), C.c_int, C.c_int, vp, vp, vp]
     L.pqp_update_limits_device.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp]
@@ -91,6 +94,10 @@ def load():
                                       [C.c_double, C.c_int, C.c_int] + [vp] * 6 + [C.POINTER(Stats)])
     L.pqp_plan_batch_device_sets.argtypes = ([vp] + [C.c_int] * 7 + [vp] * 11 + [C.c_double, C.c_int, C.c_int] +
                                              [vp] * 7 + [C.POINTER(Stats)])
+    L.pqp_plan_batch_forms.argtypes = ([vp, C.c_int, C.c_int, C.c_int] + [vp] * 11 + [C.c_double, C.c_int, C.c_int] +
+                                       [vp] * 6 + [C.POINTER(Stats)])
+    L.pqp_plan_batch_device_forms.argtypes = ([vp] + [C.c_int] * 7 + [vp] * 12 + [C.c_double, C.c_int, C.c_int] +
+                                              [vp] * 7 + [C.POINTER(Stats)])
     L.pqp_set_maps_occupancy.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap)]
     L.pqp_set_maps_occupancy_device.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap), vp]
     L.pqp_get_map.argtypes = [vp, C.c_int, vp]

@@ -283,19 +283,23 @@ static int launch_class_set(pqp_handle *h, const pqp::BatchView &bv, int n_sets,
 
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
                           const pqp_state *ref, const int32_t *keep_in, cudaStream_t st, int *launches, int form,
-                          const int32_t *set) {
+                          const int32_t *set, const int32_t *forms) {
     static_assert(kNumVariants <= PQP_MAX_VARIANTS, "class plan arrays");
     // keep_control_steps per path
     std::vector<int32_t> keepv((size_t)batch);
-    for (int b = 0; b < batch; ++b)
-        keepv[b] = form == PQP_FORM_KPC ? 4 : form == PQP_FORM_K ? 1 : keep_in ? keep_in[b] : (n[b] >= 2 ? pqp_keep_control_steps(PQP_FORM_KP, ref + off[b], n[b]) : 1);
+    for (int b = 0; b < batch; ++b) {
+        const int f = forms ? forms[b] : form;
+        keepv[b] = f == PQP_FORM_KPC ? 4 : f == PQP_FORM_K ? 1 : keep_in ? keep_in[b] : (n[b] >= 2 ? pqp_keep_control_steps(PQP_FORM_KP, ref + off[b], n[b]) : 1);
+    }
     const int n_sets = set ? (int)h->dsets.size() : 1;
-    // The plan (segment per path, longest-first order inside a segment) only depends on (n, keep, set): a caller that
-    // solves batches of the same shape back to back reuses it, and the order array already on the device with it.
+    // The plan (segment per path, longest-first order inside a segment) only depends on (n, keep, set, formulation): a
+    // caller that solves batches of the same shape back to back reuses it, and the order array already on the device
+    // with it.
     pqp_handle::ClassPlan &pl = h->plan;
     const bool same = pl.valid && pl.form == form && pl.skip == (int)skip_mask() && pl.n.size() == (size_t)batch &&
                       std::equal(pl.n.begin(), pl.n.end(), n) && pl.keep == keepv && pl.n_sets == n_sets &&
-                      (set ? pl.set.size() == (size_t)batch && std::equal(pl.set.begin(), pl.set.end(), set) : pl.set.empty());
+                      (set ? pl.set.size() == (size_t)batch && std::equal(pl.set.begin(), pl.set.end(), set) : pl.set.empty()) &&
+                      (forms ? pl.forms.size() == (size_t)batch && std::equal(pl.forms.begin(), pl.forms.end(), forms) : pl.forms.empty());
     if (!same) {
         // the pinned order array may still be the source of an earlier asynchronous upload
         PQP_CUDA(cudaStreamSynchronize(st));
@@ -308,10 +312,11 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
         pl.smem.assign((size_t)G + 1, 0);
         for (int b = 0; b < batch; ++b) {
             const int s = set ? set[b] : 0;
-            if (s < 0 || s >= n_sets) { seg[b] = G; pl.count[G]++; continue; }
+            const int f = forms ? forms[b] : form;
+            if (s < 0 || s >= n_sets || (forms && !pqp::form_in_mask(f, 7))) { seg[b] = G; pl.count[G]++; continue; }
             int v;
             size_t need;
-            class_for(h, n[b], keepv[b], &v, &need, form);
+            class_for(h, n[b], keepv[b], &v, &need, f);
             seg[b] = s * kNumVariants + v;
             pl.smem[seg[b]] = std::max(pl.smem[seg[b]], need);
             pl.count[seg[b]]++;
@@ -332,6 +337,8 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
         pl.keep = keepv;
         if (set) pl.set.assign(set, set + batch);
         else pl.set.clear();
+        if (forms) pl.forms.assign(forms, forms + batch);
+        else pl.forms.clear();
         pl.n_sets = n_sets;
         pl.n_reject = pl.count[G];
         pl.skip = (int)skip_mask();
@@ -370,52 +377,36 @@ struct DispatchArgs {
     const int32_t *set;        // [batch] parameter set of every path, NULL: set 0
     int n_sets;                // sets launched: a path whose set lies outside [0, n_sets) is answered here; 1 without `set`
     int32_t *hist;             // [n_sets * nv * ncols + n_sets * nv] histogram and bases in global memory, NULL: shared
+    const int32_t *form_of;    // pqp_dispatch_forms_kernel: [batch] formulation of every path
+    int form_mask;             //   and the formulations launched (1 << PQP_FORM_*)
 };
 
 __global__ void pqp_fill_kernel(int32_t *p, size_t n, int32_t value) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = value;
 }
 
-__global__ void __launch_bounds__(kDispatchThreads)
-pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
-    // [n_sets * nv * ncols] paths per (set, class, longest-first length bucket), then [n_sets * nv] bases: in shared
-    // memory for one set, in global memory (a.hist) for several
-    extern __shared__ int32_t hist_s[];
-    __shared__ int32_t warp_sum[kDispatchThreads / 32];
-    int32_t *hist = a.hist ? a.hist : hist_s;
-    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    int32_t *base = hist + nb;
-    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
-    if (tid == 0) a.n_view[a.batch] = 0;
-    __syncthreads();
-    for (int b = tid; b < a.batch; b += kDispatchThreads) {
-        const int n = a.n_points[b], off = a.offsets[b];
-        a.n_view[b] = n;
-        const int s = a.set ? a.set[b] : 0;
-        const bool set_ok = s >= 0 && s < a.n_sets;
-        const int keep = set_ok ? pqp::keep_control_steps(a.form, a.ref + off, n) : 0;
-        const int v = set_ok ? pqp::dispatch_class(a.table, a.ncols, a.form, n, keep, a.max_n, a.min_keep, a.max_keep) : -1;
-        int key = -1;
-        if (v >= 0) {
-            key = pqp::dispatch_key(s, v - a.v0, a.nv, a.ncols, n);
-            atomicAdd(&hist[key], 1);
-        } else {
-            a.status[b] = PQP_INVALID_PROBLEM;
-            a.iters[b] = 0;
-            const double qnan = nan("");
-            for (int i = 0; i < n; ++i) {
-                pqp_state &o = a.out_states[off + i];
-                o.x = o.y = o.z = o.k = o.s = qnan;
-                o.v = o.a = 0.0;
-                if (a.out_frenet) {
-                    double *f = a.out_frenet + 3 * (size_t)(off + i);
-                    f[0] = f[1] = f[2] = qnan;
-                }
-            }
+// A path the dispatch does not launch, answered as a kernel answers a path it cannot take.
+__device__ __forceinline__ void dispatch_reject(const DispatchArgs &a, int b, int n, int off) {
+    a.status[b] = PQP_INVALID_PROBLEM;
+    a.iters[b] = 0;
+    const double qnan = nan("");
+    for (int i = 0; i < n; ++i) {
+        pqp_state &o = a.out_states[off + i];
+        o.x = o.y = o.z = o.k = o.s = qnan;
+        o.v = o.a = 0.0;
+        if (a.out_frenet) {
+            double *f = a.out_frenet + 3 * (size_t)(off + i);
+            f[0] = f[1] = f[2] = qnan;
         }
-        a.key[b] = key;
     }
-    __syncthreads();
+}
+
+// The second half of both dispatch kernels, once every path's key is in a.key and counted in hist[0, nsv * ncols):
+// exclusive prefix of the histogram, then the scatter into the order segments (nsv of them, `batch` entries each).
+__device__ __forceinline__ void dispatch_scatter(const DispatchArgs &a, int32_t *hist, int nsv, int ncols,
+                                                 int32_t *warp_sum) {
+    const int nb = nsv * ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    int32_t *base = hist + nb;
     // exclusive prefix of the histogram: every thread owns a run of consecutive buckets
     const int per = (nb + kDispatchThreads - 1) / kDispatchThreads, lo = min(tid * per, nb), hi = min(lo + per, nb);
     int sum = 0;
@@ -444,25 +435,82 @@ pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
         run += c;
     }
     __syncthreads();
-    for (int r = tid; r < nsv; r += kDispatchThreads) base[r] = hist[r * a.ncols];
+    for (int r = tid; r < nsv; r += kDispatchThreads) base[r] = hist[r * ncols];
     __syncthreads();
     for (int b = tid; b < a.batch; b += kDispatchThreads) {
         const int key = a.key[b];
         if (key < 0) continue;
-        const int r = key / a.ncols;
+        const int r = key / ncols;
         a.order[(size_t)r * a.batch + (atomicAdd(&hist[key], 1) - base[r])] = b;
     }
+}
+
+__global__ void __launch_bounds__(kDispatchThreads)
+pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
+    // [n_sets * nv * ncols] paths per (set, class, longest-first length bucket), then [n_sets * nv] bases: in shared
+    // memory for one set, in global memory (a.hist) for several
+    extern __shared__ int32_t hist_s[];
+    __shared__ int32_t warp_sum[kDispatchThreads / 32];
+    int32_t *hist = a.hist ? a.hist : hist_s;
+    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x;
+    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
+    if (tid == 0) a.n_view[a.batch] = 0;
+    __syncthreads();
+    for (int b = tid; b < a.batch; b += kDispatchThreads) {
+        const int n = a.n_points[b], off = a.offsets[b];
+        a.n_view[b] = n;
+        const int s = a.set ? a.set[b] : 0;
+        const bool set_ok = s >= 0 && s < a.n_sets;
+        const int keep = set_ok ? pqp::keep_control_steps(a.form, a.ref + off, n) : 0;
+        const int v = set_ok ? pqp::dispatch_class(a.table, a.ncols, a.form, n, keep, a.max_n, a.min_keep, a.max_keep) : -1;
+        int key = -1;
+        if (v >= 0) {
+            key = pqp::dispatch_key(s, v - a.v0, a.nv, a.ncols, n);
+            atomicAdd(&hist[key], 1);
+        } else {
+            dispatch_reject(a, b, n, off);
+        }
+        a.key[b] = key;
+    }
+    __syncthreads();
+    dispatch_scatter(a, hist, nsv, a.ncols, warp_sum);
+}
+
+// The dispatch over per-path formulations: every path looks its class up in the table of its own formulation
+// (t.table[a.form_of[b]]) and is keyed by (set, class of the whole variant space, length) with
+// pqp::dispatch_key_forms; a.nv = every class, a.ncols = the stride shared by the formulations.  The rest is
+// pqp_dispatch_kernel's.
+__global__ void __launch_bounds__(kDispatchThreads)
+pqp_dispatch_forms_kernel(const __grid_constant__ DispatchArgs a, const __grid_constant__ pqp::FormTables t) {
+    extern __shared__ int32_t hist_s[];
+    __shared__ int32_t warp_sum[kDispatchThreads / 32];
+    int32_t *hist = a.hist ? a.hist : hist_s;
+    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x;
+    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
+    if (tid == 0) a.n_view[a.batch] = 0;
+    __syncthreads();
+    for (int b = tid; b < a.batch; b += kDispatchThreads) {
+        const int n = a.n_points[b], off = a.offsets[b];
+        a.n_view[b] = n;
+        const int s = a.set ? a.set[b] : 0;
+        const int f = a.form_of[b];
+        const int keep = pqp::form_in_mask(f, a.form_mask) ? pqp::keep_control_steps(f, a.ref + off, n) : 0;
+        const int key = pqp::dispatch_key_forms(t, a.form_mask, f, s, a.n_sets, n, keep, a.min_keep, a.max_keep, a.nv,
+                                                a.ncols);
+        if (key >= 0) atomicAdd(&hist[key], 1);
+        else dispatch_reject(a, b, n, off);
+        a.key[b] = key;
+    }
+    __syncthreads();
+    dispatch_scatter(a, hist, nsv, a.ncols, warp_sum);
 }
 
 namespace {
 size_t dispatch_smem(int nv, int ncols) { return ((size_t)nv * ncols + nv) * sizeof(int32_t); }
 
-// Which classes the stated bounds reach, the shortest path each of them can get and the shared memory it needs: every
-// (n, keep) inside the bounds, as class_for maps it.  Cached for the last bounds.
-void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max_keep) {
-    pqp_handle::DispatchLaunches &d = h->disp;
-    if (d.valid && d.form == form && d.max_n == max_n && d.min_keep == min_keep && d.max_keep == max_keep) return;
-    d = pqp_handle::DispatchLaunches();
+// Which classes of `form` the stated bounds reach, the shortest path each of them can get and the shared memory it
+// needs: every (n, keep) inside the bounds, as class_for maps it.  Adds to `d` (min_n starts at INT32_MAX).
+void reach_classes(const pqp_handle *h, pqp_handle::DispatchLaunches &d, int form, int max_n, int min_keep, int max_keep) {
     const int ncols = h->cls_ncols[form];
     const int col_hi = max_n > 0 ? std::min(max_n, ncols - 1) : ncols - 1;
     int r_lo = 0, r_hi = pqp::kTableKeepRows - 1;
@@ -472,7 +520,6 @@ void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max
     } else {
         r_lo = r_hi = pqp::keep_control_steps(form, nullptr, 0) - 1;
     }
-    for (int v = 0; v < kNumVariants; ++v) d.min_n[v] = INT32_MAX;
     for (int r = r_lo; r <= r_hi; ++r)
         for (int n = 0; n <= col_hi; ++n) {
             int v;
@@ -482,7 +529,32 @@ void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max
             d.smem[v] = std::max(d.smem[v], need);
             d.min_n[v] = std::min(d.min_n[v], n);
         }
+}
+
+// The classes one formulation's bounds reach, cached for the last bounds.
+void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max_keep) {
+    pqp_handle::DispatchLaunches &d = h->disp;
+    if (d.valid && d.form == form && d.max_n == max_n && d.min_keep == min_keep && d.max_keep == max_keep) return;
+    d = pqp_handle::DispatchLaunches();
+    for (int v = 0; v < kNumVariants; ++v) d.min_n[v] = INT32_MAX;
+    reach_classes(h, d, form, max_n, min_keep, max_keep);
     d.form = form; d.max_n = max_n; d.min_keep = min_keep; d.max_keep = max_keep;
+    d.valid = true;
+}
+
+// The same over the formulations of `form_mask`, formulation f bounded by max_n[f]; cached for the last (mask, bounds)
+// in a cache of its own, so that the single-formulation entries keep theirs.  Classes belong to one formulation each,
+// so every class gets exactly what dispatch_launches gives it for its formulation alone.
+void dispatch_launches_forms(pqp_handle *h, int form_mask, const int max_n[3], int min_keep, int max_keep) {
+    pqp_handle::DispatchLaunches &d = h->disp_forms;
+    if (d.valid && d.form == form_mask && std::equal(max_n, max_n + 3, d.max_n_form) && d.min_keep == min_keep &&
+        d.max_keep == max_keep)
+        return;
+    d = pqp_handle::DispatchLaunches();
+    for (int v = 0; v < kNumVariants; ++v) d.min_n[v] = INT32_MAX;
+    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC})
+        if (pqp::form_in_mask(f, form_mask)) reach_classes(h, d, f, max_n[f], min_keep, max_keep);
+    d.form = form_mask; std::copy(max_n, max_n + 3, d.max_n_form); d.min_keep = min_keep; d.max_keep = max_keep;
     d.valid = true;
 }
 }  // namespace
@@ -544,6 +616,77 @@ int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int b
             const int g = s * kNumVariants + v;
             count[g] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
             start[g] = (s * nv + v - v0) * batch;
+            smem[g] = d.smem[v];
+        }
+    const int rc = launch_class_set(h, dv, n_sets, count.data(), start.data(), smem.data(), order, st, launches);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaMemcpyAsync(bv.status, h->d_disp_status, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (bv.iters)
+        PQP_CUDA(cudaMemcpyAsync(bv.iters, h->d_disp_iters, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    return PQP_OK;
+}
+
+int pqp_launch_dispatch_forms(pqp_handle *h, const pqp::BatchView &bv, int form_mask, int batch, int total,
+                              const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
+                              const int32_t *d_form, const int32_t *d_set, int n_param_sets) {
+    dispatch_launches_forms(h, form_mask, max_n, min_keep, max_keep);
+    int ncols = 0;
+    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) ncols = std::max(ncols, h->cls_ncols[f]);
+    const int nv = kNumVariants;
+    int n_sets = 1;
+    if (d_set) {
+        n_sets = (int)h->dsets.size();
+        if (n_param_sets > 0) n_sets = std::min(n_sets, n_param_sets);
+    }
+    // order segments over every class (and, with a set index, the histogram) in grow-only scratch of their own: the
+    // single-formulation entries keep their buffers and layout
+    if (n_sets > h->form_cap) {
+        int cap = 1;
+        while (cap < n_sets) cap *= 2;
+        int32_t *o = nullptr, *hs = nullptr;
+        PQP_CUDA(cudaMalloc(&o, (size_t)cap * nv * h->max_batch * sizeof(int32_t)));
+        if (cudaMalloc(&hs, (size_t)cap * nv * (ncols + 1) * sizeof(int32_t)) != cudaSuccess) {
+            cudaFree(o);
+            set_err("pqp_launch_dispatch_forms: cudaMalloc of the formulation sort scratch failed");
+            return PQP_ERR_CUDA;
+        }
+        if (h->d_form_order) { h->retired.push_back(h->d_form_order); h->retired.push_back(h->d_form_hist); }
+        h->d_form_order = o; h->d_form_hist = hs; h->form_cap = cap;
+    }
+    int32_t *order = h->d_form_order, *hist = d_set ? h->d_form_hist : nullptr;
+    const size_t n_order = (size_t)n_sets * nv * batch;
+    pqp_fill_kernel<<<(unsigned)std::min<size_t>((n_order + 255) / 256, 1024), 256, 0, st>>>(order, n_order, batch);
+    PQP_CUDA(cudaGetLastError());
+    DispatchArgs a;
+    a.table = nullptr;
+    a.ncols = ncols; a.form = -1; a.v0 = 0; a.nv = nv;
+    a.max_n = 0; a.min_keep = min_keep; a.max_keep = max_keep; a.batch = batch;
+    a.n_points = bv.n_points; a.offsets = bv.offsets; a.ref = bv.ref;
+    a.out_states = bv.out_states; a.out_frenet = bv.out_frenet; a.status = h->d_disp_status; a.iters = h->d_disp_iters;
+    a.n_view = h->d_disp_n; a.key = h->d_disp_key; a.order = order;
+    a.set = d_set; a.n_sets = n_sets; a.hist = hist;
+    a.form_of = d_form; a.form_mask = form_mask;
+    pqp::FormTables t;
+    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
+        t.table[f] = h->d_cls_table + h->cls_off[f];
+        t.ncols[f] = h->cls_ncols[f];
+        t.max_n[f] = max_n[f];
+    }
+    pqp_dispatch_forms_kernel<<<1, kDispatchThreads, hist ? 0 : dispatch_smem(nv, ncols), st>>>(a, t);
+    PQP_CUDA(cudaGetLastError());
+    if (launches) *launches += 2;
+    pqp::BatchView dv = bv;
+    dv.n_points = h->d_disp_n; dv.status = h->d_disp_status; dv.iters = h->d_disp_iters;
+    // grid per reached (set, class) exactly as pqp_launch_dispatch sizes it for the class's formulation alone
+    std::vector<int> count((size_t)n_sets * nv, 0), start((size_t)n_sets * nv, 0);
+    std::vector<size_t> smem((size_t)n_sets * nv, 0);
+    const pqp_handle::DispatchLaunches &d = h->disp_forms;
+    for (int s = 0; s < n_sets; ++s)
+        for (int v = 0; v < nv; ++v) {
+            if (!d.reach[v]) continue;
+            const int g = s * nv + v;
+            count[g] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
+            start[g] = g * batch;
             smem[g] = d.smem[v];
         }
     const int rc = launch_class_set(h, dv, n_sets, count.data(), start.data(), smem.data(), order, st, launches);
@@ -638,6 +781,7 @@ void pqp_destroy(pqp_handle *h) {
     cudaFree(h->d_cls_table); cudaFree(h->d_disp_order); cudaFree(h->d_disp_key);
     cudaFree(h->d_disp_n); cudaFree(h->d_disp_status); cudaFree(h->d_disp_iters);
     cudaFree(h->d_set_order); cudaFree(h->d_set_hist);
+    cudaFree(h->d_form_order); cudaFree(h->d_form_hist);
     for (void *p : h->retired) cudaFree(p);
     cudaFreeHost(h->h_off); cudaFreeHost(h->h_order);
     cudaFree(h->d_gen); cudaFreeHost(h->h_gen);
@@ -732,6 +876,7 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
     {
         std::vector<int8_t> all, tab;
         size_t smem = 0;
+        int ncols_max = 0;
         for (int form : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
             int v0, v1;
             form_range(form, &v0, &v1);
@@ -739,10 +884,13 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
             h->cls_off[form] = (int)all.size();
             all.insert(all.end(), tab.begin(), tab.end());
             smem = std::max(smem, dispatch_smem(v1 - v0, h->cls_ncols[form]));
+            ncols_max = std::max(ncols_max, h->cls_ncols[form]);
         }
         PQP_TRY(cudaMalloc(&h->d_cls_table, all.size()));
         PQP_TRY(cudaMemcpy(h->d_cls_table, all.data(), all.size(), cudaMemcpyHostToDevice));
         PQP_TRY(cudaFuncSetAttribute(pqp_dispatch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PQP_TRY(cudaFuncSetAttribute(pqp_dispatch_forms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)dispatch_smem(kNumVariants, ncols_max)));
         PQP_TRY(cudaMalloc(&h->d_disp_order, (size_t)kNumKp * B * sizeof(int32_t)));
         PQP_TRY(cudaMalloc(&h->d_disp_key, B * sizeof(int32_t)));
         PQP_TRY(cudaMalloc(&h->d_disp_n, (B + 1) * sizeof(int32_t)));
@@ -1032,6 +1180,52 @@ int pqp_solve_batch_device_dispatch_sets(pqp_handle *h, int formulation, int bat
     return PQP_OK;
 }
 
+int pqp_solve_batch_device_dispatch_forms(pqp_handle *h, int batch, int total_points, int max_n_points, int min_keep,
+                                          int max_keep, int n_param_sets, int form_mask, const int32_t *d_n_points,
+                                          const int32_t *d_offsets, const pqp_state *d_ref,
+                                          const pqp_station_bounds *d_bounds, const double *d_x0,
+                                          const double *d_end_heading, const double *d_max_k, const double *d_max_kp,
+                                          const int32_t *d_param_index, const int32_t *d_formulation,
+                                          pqp_state *d_out_states, double *d_out_frenet, int32_t *d_status,
+                                          int32_t *d_iters, void *stream, pqp_stats *stats) {
+    if (!h || batch < 0 || n_param_sets < 0 || form_mask < 0 || form_mask > 7 || !d_n_points || !d_offsets || !d_ref ||
+        !d_bounds || !d_x0 || !d_end_heading || !d_formulation || !d_out_states || !d_status) {
+        set_err("pqp_solve_batch_device_dispatch_forms: bad argument");
+        return PQP_ERR_ARG;
+    }
+    const int mask = form_mask ? form_mask : 7;
+    if (pqp::form_in_mask(PQP_FORM_KPC, mask) && (!d_max_k || !d_max_kp)) {
+        set_err("a form_mask with \"KPC\" needs d_max_k and d_max_kp (pqp_update_limits_device)");
+        return PQP_ERR_ARG;
+    }
+    if (batch == 0) return PQP_OK;
+    if (batch > h->max_batch || total_points > h->max_total) {
+        set_err("batch / total_points exceed what the handle was created for (workspace size)");
+        return PQP_ERR_CAPACITY;
+    }
+    PQP_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    pqp::BatchView bv;
+    bv.batch = batch; bv.n_points = d_n_points; bv.offsets = d_offsets; bv.ref = d_ref; bv.bounds = d_bounds;
+    bv.x0 = d_x0; bv.end_heading = d_end_heading; bv.out_states = d_out_states; bv.out_frenet = d_out_frenet;
+    bv.status = d_status; bv.iters = d_iters; bv.workspace = h->d_ws; bv.debug = nullptr;
+    bv.max_k = d_max_k; bv.max_kp = d_max_kp;
+    if (stats) PQP_CUDA(cudaEventRecord(h->ev[0], st));
+    int launches = 0;
+    const int max_n[3] = {max_n_points, max_n_points, max_n_points};
+    int rc = pqp_launch_dispatch_forms(h, bv, mask, batch, total_points, max_n, min_keep, max_keep, st, &launches,
+                                       d_formulation, d_param_index, n_param_sets);
+    if (rc != PQP_OK) return rc;
+    if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        PQP_CUDA(cudaEventRecord(h->ev[1], st));
+        PQP_CUDA(cudaEventSynchronize(h->ev[1]));
+        PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
+        stats->kernel_launches = launches;
+    }
+    return PQP_OK;
+}
+
 int pqp_class_table(int formulation, int smem_optin, int8_t *table, int capacity, int *ncols) {
     if ((formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) || !ncols) return PQP_ERR_ARG;
     pqp_handle fake;
@@ -1178,6 +1372,23 @@ static int solve_batch_generic(pqp_handle *h, int formulation, int batch, const 
     return PQP_OK;
 }
 
+}  // extern "C"
+
+// PQP_GENERIC_KPC=1 / PQP_GENERIC_K=1 (diagnostics): route "KPC" / "K" through the host-assembled generic kernel
+// (round 1's path for them) instead of their thread-per-station classes
+static bool generic_form(int formulation) {
+    static const bool generic_kpc = [] { const char *e = getenv("PQP_GENERIC_KPC"); return e && *e == '1'; }();
+    static const bool generic_k = [] { const char *e = getenv("PQP_GENERIC_K"); return e && *e == '1'; }();
+    return (formulation == PQP_FORM_KPC && generic_kpc) || (formulation == PQP_FORM_K && generic_k);
+}
+static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *forms, int batch, const int32_t *n_points,
+                               const pqp_state *ref, const pqp_station_bounds *bounds, const double *x0,
+                               const double *end_heading, const double *max_k, const double *max_kp,
+                               const int32_t *param_index, pqp_state *out_states, double *out_frenet, int32_t *status,
+                               int32_t *iters, pqp_stats *stats);
+
+extern "C" {
+
 int pqp_solve_batch(pqp_handle *h, int formulation, int batch, const int32_t *n_points, const pqp_state *ref,
                     const pqp_station_bounds *bounds, const double *x0, const double *end_heading,
                     const double *max_k, const double *max_kp, pqp_state *out_states, double *out_frenet,
@@ -1204,13 +1415,7 @@ int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch, const int32_
         set_err("KPC needs max_k and max_kp (ReferencePath::getMaxKList / getMaxKpList; pqp_update_limits)");
         return PQP_ERR_ARG;
     }
-    // PQP_GENERIC_KPC=1 / PQP_GENERIC_K=1 (diagnostics): route "KPC" / "K" through the host-assembled generic kernel
-    // (round 1's path for them) instead of their thread-per-station classes
-    static const bool generic_kpc = [] { const char *e = getenv("PQP_GENERIC_KPC"); return e && *e == '1'; }();
-    static const bool generic_k = [] { const char *e = getenv("PQP_GENERIC_K"); return e && *e == '1'; }();
-    const bool kpc_classes = formulation == PQP_FORM_KPC && !generic_kpc;
-    const bool k_classes = formulation == PQP_FORM_K && !generic_k;
-    if (formulation != PQP_FORM_KP && !kpc_classes && !k_classes) {
+    if (generic_form(formulation)) {
         if (param_index) {
             set_err("the host-assembled diagnostic path (PQP_GENERIC_K / PQP_GENERIC_KPC) takes no parameter-set index");
             return PQP_ERR_UNSUPPORTED;
@@ -1218,6 +1423,55 @@ int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch, const int32_
         return solve_batch_generic(h, formulation, batch, n_points, ref, bounds, x0, end_heading, max_k, max_kp, out_states,
                                    out_frenet, status, iters, stats);
     }
+    return solve_batch_classes(h, formulation, nullptr, batch, n_points, ref, bounds, x0, end_heading, max_k, max_kp,
+                               param_index, out_states, out_frenet, status, iters, stats);
+}
+
+int pqp_solve_batch_forms(pqp_handle *h, int batch, const int32_t *n_points, const pqp_state *ref,
+                          const pqp_station_bounds *bounds, const double *x0, const double *end_heading,
+                          const double *max_k, const double *max_kp, const int32_t *param_index,
+                          const int32_t *formulation, pqp_state *out_states, double *out_frenet, int32_t *status,
+                          int32_t *iters, pqp_stats *stats) {
+    if (!h || batch < 0 ||
+        (batch > 0 && (!n_points || !ref || !bounds || !x0 || !end_heading || !formulation || !out_states || !status))) {
+        set_err("pqp_solve_batch_forms: bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (stats) memset(stats, 0, sizeof(*stats));
+    bool any_kpc = false, any_generic = false;
+    for (int b = 0; b < batch; ++b) {
+        any_kpc |= formulation[b] == PQP_FORM_KPC;
+        any_generic |= pqp::form_in_mask(formulation[b], 7) && generic_form(formulation[b]);
+    }
+    if (any_kpc && (!max_k || !max_kp)) {
+        set_err("a \"KPC\" path needs max_k and max_kp (ReferencePath::getMaxKList / getMaxKpList; pqp_update_limits)");
+        return PQP_ERR_ARG;
+    }
+    if (any_generic) {
+        set_err("the host-assembled diagnostic path (PQP_GENERIC_K / PQP_GENERIC_KPC) takes no per-path formulation");
+        return PQP_ERR_UNSUPPORTED;
+    }
+    if (batch == 0) return PQP_OK;
+    if (h->defer_sync) {
+        set_err("pqp_solve_batch_forms: no per-path formulation on a multi-device handle");
+        return PQP_ERR_UNSUPPORTED;
+    }
+    return solve_batch_classes(h, PQP_FORM_KP, formulation, batch, n_points, ref, bounds, x0, end_heading, max_k, max_kp,
+                               param_index, out_states, out_frenet, status, iters, stats);
+}
+
+}  // extern "C"
+
+// The host-buffer solve on the kernel classes: pqp_solve_batch_sets (forms NULL: `formulation` for every path) and
+// pqp_solve_batch_forms (forms [batch]: every path's own; one that is not a PQP_FORM_* is rejected like an out-of-range
+// set index).  Arguments checked by the callers.
+static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *forms, int batch, const int32_t *n_points,
+                               const pqp_state *ref, const pqp_station_bounds *bounds, const double *x0,
+                               const double *end_heading, const double *max_k, const double *max_kp,
+                               const int32_t *param_index, pqp_state *out_states, double *out_frenet, int32_t *status,
+                               int32_t *iters, pqp_stats *stats) {
+    bool kpc_classes = formulation == PQP_FORM_KPC;
+    for (int b = 0; forms && b < batch; ++b) kpc_classes |= forms[b] == PQP_FORM_KPC;
     if (batch > h->max_batch) {
         set_err("batch exceeds the handle's max_batch");
         return PQP_ERR_CAPACITY;
@@ -1241,11 +1495,12 @@ int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch, const int32_
         if (total > h->max_total) { set_err("station count exceeds the handle's max_total_points"); return PQP_ERR_CAPACITY; }
         h->h_off[b + 1] = (int32_t)total;
         const int s = param_index ? param_index[b] : 0;
-        if (s < 0 || s >= n_sets) { cls[b] = G; need_b[b] = 0; continue; }
-        const int keep = (n >= 2) ? pqp_keep_control_steps(formulation, ref + h->h_off[b], n) : 1;
+        const int f = forms ? forms[b] : formulation;
+        if (s < 0 || s >= n_sets || (forms && !pqp::form_in_mask(f, 7))) { cls[b] = G; need_b[b] = 0; continue; }
+        const int keep = (n >= 2) ? pqp_keep_control_steps(f, ref + h->h_off[b], n) : 1;
         int v;
         size_t need;
-        class_for(h, n, keep, &v, &need, formulation);
+        class_for(h, n, keep, &v, &need, f);
         cls[b] = s * kNumVariants + v;
         need_b[b] = need;
     }
@@ -1479,4 +1734,3 @@ int pqp_solve_batch_sets(pqp_handle *h, int formulation, int batch, const int32_
     return PQP_OK;
 }
 
-}  // extern "C"

@@ -58,4 +58,30 @@ PQP_HD int dispatch_key(int set, int cls, int nv, int ncols, int n) {
     return (set * nv + cls) * ncols + (ncols - 1 - col);
 }
 
+// The dispatch over per-path formulations (the _forms entries): the class table, its ncols and the length bound of
+// every formulation, indexed by PQP_FORM_*.  max_n[f] = 0: unknown, as for dispatch_class.
+struct FormTables {
+    const int8_t *table[3];
+    int ncols[3];
+    int max_n[3];
+};
+
+// Whether `form` is a formulation and one of the `form_mask` bits (1 << PQP_FORM_*).
+PQP_HD bool form_in_mask(int form, int form_mask) {
+    return form >= 0 && form <= 2 && ((form_mask >> form) & 1);
+}
+
+// Sort key of the per-path-formulation dispatch for a path of `form`, n stations, keep_control_steps `keep` and
+// parameter set `set`: histogram bucket (set * n_variants + v) * ncols + the longest-first length bucket, where v is the
+// class index (global over the formulations, 0 .. n_variants - 1) the formulation's own table gives, and ncols is a
+// stride shared by every formulation (>= each table's ncols).  The order segment of the path is key / ncols, its class
+// (key / ncols) % n_variants.  -1 (no key: PQP_INVALID_PROBLEM) when the formulation is unknown or outside form_mask,
+// the set lies outside [0, n_sets), or the path lies outside its formulation's bounds.
+PQP_HD int dispatch_key_forms(const FormTables &t, int form_mask, int form, int set, int n_sets, int n, int keep,
+                              int min_keep, int max_keep, int n_variants, int ncols) {
+    if (!form_in_mask(form, form_mask) || set < 0 || set >= n_sets) return -1;
+    const int v = dispatch_class(t.table[form], t.ncols[form], form, n, keep, t.max_n[form], min_keep, max_keep);
+    return v < 0 ? -1 : dispatch_key(set, v, n_variants, ncols, n);
+}
+
 }  // namespace pqp

@@ -16,6 +16,7 @@
 
 #include "pqp_edt_core.cuh"
 #include "pqp_env_core.cuh"
+#include "pqp_dispatch.h"
 #include "pqp_handle.h"
 
 namespace {
@@ -1052,6 +1053,12 @@ struct ChainIO {
     const int32_t *map_index;       // [batch] map of every path (bounds and collision check), NULL: map 0
     SetIndex set;                   // parameter set of every path (device index, NULL: set 0) and the sets it may name
     const int32_t *h_set;           // host copy of set.index (host class plan), else NULL
+    // per-path formulation (the _forms entries; `formulation` is then unused): the host array (host class plan) or the
+    // device array (device dispatch), NULL both without; form_mask = the formulations a path may name (1 << PQP_FORM_*)
+    // and max_n_form[f] the longest path of formulation f the device dispatch takes
+    const int32_t *h_form = nullptr, *d_form = nullptr;
+    int form_mask = 0;
+    int max_n_form[3] = {};
     const double *x0, *end_heading;
     double spacing;
     int collision_check, max_out;
@@ -1079,9 +1086,11 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     bv.batch = c.batch; bv.n_points = e->d_nvalid; bv.offsets = c.paths.offsets; bv.ref = c.paths.ref; bv.bounds = c.bounds;
     bv.x0 = c.x0; bv.end_heading = c.end_heading; bv.out_states = c.qp_states; bv.out_frenet = nullptr;
     bv.status = c.status; bv.iters = c.iters; bv.workspace = h->d_ws; bv.debug = nullptr;
-    if (c.formulation == PQP_FORM_KPC) {
+    const bool mixed = c.h_form || c.d_form;
+    if (mixed ? pqp::form_in_mask(PQP_FORM_KPC, c.form_mask) : c.formulation == PQP_FORM_KPC) {
         // updateLimits (reference_path_impl.cpp:203-235) between updateBounds and the QP, as solveWithoutSmoothing
-        // does (path_optimizer.cpp:100-105): limits from the v, a fields of the reference states
+        // does (path_optimizer.cpp:100-105): limits from the v, a fields of the reference states.  With per-path
+        // formulations every path gets them; only the "KPC" paths read them.
         if (!h->d_max_k) {
             PQP_CUDA(cudaMalloc(&h->d_max_k, (size_t)h->max_total * sizeof(double)));
             PQP_CUDA(cudaMalloc(&h->d_max_kp, (size_t)h->max_total * sizeof(double)));
@@ -1099,7 +1108,10 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
         PQP_CUDA(cudaMemcpyAsync(nv.data(), e->d_nvalid, (size_t)c.batch * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         PQP_CUDA(cudaStreamSynchronize(st));
         rc = pqp_launch_kp_classes(h, bv, c.batch, nv.data(), h->h_off, h_ref, nullptr, st, qp_launches, c.formulation,
-                                   c.h_set);
+                                   c.h_set, c.h_form);
+    } else if (c.d_form) {
+        rc = pqp_launch_dispatch_forms(h, bv, c.form_mask, c.batch, (int)c.total, c.max_n_form, 0, 0, st, qp_launches,
+                                       c.d_form, c.set.index, c.set.n_sets);
     } else {
         rc = pqp_launch_dispatch(h, bv, c.formulation, c.batch, (int)c.total, c.max_n, 0, 0, st, qp_launches, c.set.index,
                                  c.set.n_sets);
@@ -1130,23 +1142,17 @@ int pqp_plan_batch_maps(pqp_handle *h, int formulation, int bounds_mode, int out
                                out_states, out_n, out_ok, status, iters, out_bounds, stats);
 }
 
-int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
-                        const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
-                        const int32_t *param_index, const int32_t *n_knots, const double *knots, const double *x_coef,
-                        const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
-                        int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
-                        int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
-    if (!h || batch < 0 || (batch > 0 && (!n_points || !ref || !x0 || !end_heading || !out_states || !out_n || !out_ok)) ||
-        (bounds_mode != PQP_BOUNDS_IMPROVED && bounds_mode != PQP_BOUNDS_SIMPLE) ||
-        (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
-        (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch(_maps, _sets): bad argument");
-        return PQP_ERR_ARG;
-    }
-    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch(_maps, _sets): unknown formulation");
-        return PQP_ERR_ARG;
-    }
+}  // extern "C"
+
+// The body of pqp_plan_batch_sets (forms NULL) and pqp_plan_batch_forms (forms [batch] on the host); arguments checked
+// by the callers.
+static int plan_batch_host(pqp_handle *h, int formulation, const int32_t *forms, int bounds_mode, int output_mode,
+                           int batch, const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                           const int32_t *param_index, const int32_t *n_knots, const double *knots,
+                           const double *x_coef, const double *y_coef, const double *x0, const double *end_heading,
+                           double output_spacing, int collision_check, int max_out, pqp_state *out_states,
+                           int32_t *out_n, int32_t *out_ok, int32_t *status, int32_t *iters,
+                           pqp_station_bounds *out_bounds, pqp_stats *stats) {
     if (stats) memset(stats, 0, sizeof(*stats));
     EnvState *e;
     int rc = need_map(h, &e);
@@ -1180,6 +1186,9 @@ int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int out
     c.max_n = max_n; c.total = T; c.paths = handle_paths(h, e); c.map_index = map_index ? e->d_mapidx : nullptr;
     c.set = param_index ? SetIndex{e->d_setidx, (int)h->sets.size()} : kSet0;
     c.h_set = param_index;
+    c.h_form = forms;
+    for (int b = 0; forms && b < batch; ++b)
+        if (pqp::form_in_mask(forms[b], 7)) c.form_mask |= 1 << forms[b];
     c.x0 = h->d_x0; c.end_heading = h->d_end;
     c.spacing = output_spacing; c.collision_check = collision_check; c.max_out = max_out;
     c.qp_states = h->d_out; c.dense = e->d_dense; c.out_n = e->d_nkept; c.out_ok = e->d_ok;
@@ -1230,6 +1239,52 @@ int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int out
     return PQP_OK;
 }
 
+static bool plan_args_ok(int bounds_mode, int output_mode, double output_spacing, int max_out) {
+    return (bounds_mode == PQP_BOUNDS_IMPROVED || bounds_mode == PQP_BOUNDS_SIMPLE) &&
+           (output_mode == PQP_OUTPUT_RAW || output_mode == PQP_OUTPUT_DENSIFY) &&
+           (output_mode != PQP_OUTPUT_DENSIFY || (max_out >= 1 && output_spacing > 0.0));
+}
+
+extern "C" {
+
+int pqp_plan_batch_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                        const int32_t *n_points, const pqp_state *ref, const int32_t *map_index,
+                        const int32_t *param_index, const int32_t *n_knots, const double *knots, const double *x_coef,
+                        const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
+                        int collision_check, int max_out, pqp_state *out_states, int32_t *out_n, int32_t *out_ok,
+                        int32_t *status, int32_t *iters, pqp_station_bounds *out_bounds, pqp_stats *stats) {
+    if (!h || batch < 0 || (batch > 0 && (!n_points || !ref || !x0 || !end_heading || !out_states || !out_n || !out_ok)) ||
+        !plan_args_ok(bounds_mode, output_mode, output_spacing, max_out)) {
+        pqp_set_err("pqp_plan_batch(_maps, _sets): bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
+        pqp_set_err("pqp_plan_batch(_maps, _sets): unknown formulation");
+        return PQP_ERR_ARG;
+    }
+    return plan_batch_host(h, formulation, nullptr, bounds_mode, output_mode, batch, n_points, ref, map_index,
+                           param_index, n_knots, knots, x_coef, y_coef, x0, end_heading, output_spacing,
+                           collision_check, max_out, out_states, out_n, out_ok, status, iters, out_bounds, stats);
+}
+
+int pqp_plan_batch_forms(pqp_handle *h, int bounds_mode, int output_mode, int batch, const int32_t *n_points,
+                         const pqp_state *ref, const int32_t *map_index, const int32_t *param_index,
+                         const int32_t *formulation, const int32_t *n_knots, const double *knots,
+                         const double *x_coef, const double *y_coef, const double *x0, const double *end_heading,
+                         double output_spacing, int collision_check, int max_out, pqp_state *out_states,
+                         int32_t *out_n, int32_t *out_ok, int32_t *status, int32_t *iters,
+                         pqp_station_bounds *out_bounds, pqp_stats *stats) {
+    if (!h || batch < 0 ||
+        (batch > 0 && (!n_points || !ref || !formulation || !x0 || !end_heading || !out_states || !out_n || !out_ok)) ||
+        !plan_args_ok(bounds_mode, output_mode, output_spacing, max_out)) {
+        pqp_set_err("pqp_plan_batch_forms: bad argument");
+        return PQP_ERR_ARG;
+    }
+    return plan_batch_host(h, PQP_FORM_KP, formulation, bounds_mode, output_mode, batch, n_points, ref, map_index,
+                           param_index, n_knots, knots, x_coef, y_coef, x0, end_heading, output_spacing,
+                           collision_check, max_out, out_states, out_n, out_ok, status, iters, out_bounds, stats);
+}
+
 int pqp_plan_batch(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, const int32_t *n_points,
                    const pqp_state *ref, const int32_t *n_knots, const double *knots, const double *x_coef,
                    const double *y_coef, const double *x0, const double *end_heading, double output_spacing,
@@ -1254,28 +1309,19 @@ int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, 
                                       d_out_states, d_out_n, d_out_ok, d_status, d_iters, d_out_bounds, stream, stats);
 }
 
-int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
-                               int total_points, int max_n_points, int n_param_sets, const int32_t *d_n_points,
-                               const int32_t *d_offsets, const pqp_state *d_ref, const int32_t *d_map_index,
-                               const int32_t *d_param_index, const int32_t *d_knot_offsets, const double *d_knots,
-                               const double *d_x_coef, const double *d_y_coef, const double *d_x0,
-                               const double *d_end_heading, double output_spacing, int collision_check, int max_out,
-                               pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok, int32_t *d_status,
-                               int32_t *d_iters, pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
-    if (!h || batch < 0 || total_points < 0 || n_param_sets < 0 ||
-        (batch > 0 && (!d_n_points || !d_offsets || !d_ref || !d_x0 || !d_end_heading || !d_out_states || !d_out_n ||
-                       !d_out_ok || !d_status)) ||
-        (bounds_mode != PQP_BOUNDS_IMPROVED && bounds_mode != PQP_BOUNDS_SIMPLE) ||
-        (bounds_mode == PQP_BOUNDS_IMPROVED && batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef)) ||
-        (output_mode != PQP_OUTPUT_RAW && output_mode != PQP_OUTPUT_DENSIFY) ||
-        (output_mode == PQP_OUTPUT_DENSIFY && (max_out < 1 || !(output_spacing > 0.0)))) {
-        pqp_set_err("pqp_plan_batch_device(_maps, _sets): bad argument");
-        return PQP_ERR_ARG;
-    }
-    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        pqp_set_err("pqp_plan_batch_device(_maps, _sets): unknown formulation");
-        return PQP_ERR_ARG;
-    }
+}  // extern "C"
+
+// The body of pqp_plan_batch_device_sets (d_form NULL) and pqp_plan_batch_device_forms (d_form [batch] on the device,
+// form_mask nonzero); arguments checked by the callers.
+static int plan_batch_device(pqp_handle *h, int formulation, int form_mask, const int32_t *d_form, int bounds_mode,
+                             int output_mode, int batch, int total_points, int max_n_points, int n_param_sets,
+                             const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                             const int32_t *d_map_index, const int32_t *d_param_index, const int32_t *d_knot_offsets,
+                             const double *d_knots, const double *d_x_coef, const double *d_y_coef,
+                             const double *d_x0, const double *d_end_heading, double output_spacing,
+                             int collision_check, int max_out, pqp_state *d_out_states, int32_t *d_out_n,
+                             int32_t *d_out_ok, int32_t *d_status, int32_t *d_iters,
+                             pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
     if (stats) memset(stats, 0, sizeof(*stats));
     EnvState *e;
     int rc = need_map(h, &e);
@@ -1289,7 +1335,17 @@ int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, 
     ChainIO c;
     c.formulation = formulation; c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
     // (0: the longest path any class of the formulation takes; a longer one reports PQP_INVALID_PROBLEM)
-    c.max_n = max_n_points > 0 ? max_n_points : h->cls_ncols[formulation] - 2;
+    if (d_form) {
+        // every formulation of the mask bounded as its single-formulation call bounds it; the bounds grid covers the
+        // longest of them
+        c.d_form = d_form; c.form_mask = form_mask; c.max_n = 0;
+        for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
+            c.max_n_form[f] = max_n_points > 0 ? max_n_points : h->cls_ncols[f] - 2;
+            if (pqp::form_in_mask(f, form_mask)) c.max_n = std::max(c.max_n, c.max_n_form[f]);
+        }
+    } else {
+        c.max_n = max_n_points > 0 ? max_n_points : h->cls_ncols[formulation] - 2;
+    }
     c.total = (size_t)total_points;
     c.paths = PathsView{d_n_points, d_offsets, d_ref, d_knot_offsets, d_knots, d_x_coef, d_y_coef};
     c.map_index = d_map_index;
@@ -1315,6 +1371,65 @@ int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, 
         stats->kernel_launches = 2 + qp_launches;
     }
     return PQP_OK;
+}
+
+static bool plan_device_args_ok(int bounds_mode, int output_mode, int batch, const int32_t *d_knot_offsets,
+                                const double *d_knots, const double *d_x_coef, const double *d_y_coef,
+                                double output_spacing, int max_out) {
+    return plan_args_ok(bounds_mode, output_mode, output_spacing, max_out) &&
+           !(bounds_mode == PQP_BOUNDS_IMPROVED && batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef));
+}
+
+extern "C" {
+
+int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch,
+                               int total_points, int max_n_points, int n_param_sets, const int32_t *d_n_points,
+                               const int32_t *d_offsets, const pqp_state *d_ref, const int32_t *d_map_index,
+                               const int32_t *d_param_index, const int32_t *d_knot_offsets, const double *d_knots,
+                               const double *d_x_coef, const double *d_y_coef, const double *d_x0,
+                               const double *d_end_heading, double output_spacing, int collision_check, int max_out,
+                               pqp_state *d_out_states, int32_t *d_out_n, int32_t *d_out_ok, int32_t *d_status,
+                               int32_t *d_iters, pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
+    if (!h || batch < 0 || total_points < 0 || n_param_sets < 0 ||
+        (batch > 0 && (!d_n_points || !d_offsets || !d_ref || !d_x0 || !d_end_heading || !d_out_states || !d_out_n ||
+                       !d_out_ok || !d_status)) ||
+        !plan_device_args_ok(bounds_mode, output_mode, batch, d_knot_offsets, d_knots, d_x_coef, d_y_coef,
+                             output_spacing, max_out)) {
+        pqp_set_err("pqp_plan_batch_device(_maps, _sets): bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
+        pqp_set_err("pqp_plan_batch_device(_maps, _sets): unknown formulation");
+        return PQP_ERR_ARG;
+    }
+    return plan_batch_device(h, formulation, 0, nullptr, bounds_mode, output_mode, batch, total_points, max_n_points,
+                             n_param_sets, d_n_points, d_offsets, d_ref, d_map_index, d_param_index, d_knot_offsets,
+                             d_knots, d_x_coef, d_y_coef, d_x0, d_end_heading, output_spacing, collision_check, max_out,
+                             d_out_states, d_out_n, d_out_ok, d_status, d_iters, d_out_bounds, stream, stats);
+}
+
+int pqp_plan_batch_device_forms(pqp_handle *h, int bounds_mode, int output_mode, int batch, int total_points,
+                                int max_n_points, int n_param_sets, int form_mask, const int32_t *d_n_points,
+                                const int32_t *d_offsets, const pqp_state *d_ref, const int32_t *d_map_index,
+                                const int32_t *d_param_index, const int32_t *d_formulation,
+                                const int32_t *d_knot_offsets, const double *d_knots, const double *d_x_coef,
+                                const double *d_y_coef, const double *d_x0, const double *d_end_heading,
+                                double output_spacing, int collision_check, int max_out, pqp_state *d_out_states,
+                                int32_t *d_out_n, int32_t *d_out_ok, int32_t *d_status, int32_t *d_iters,
+                                pqp_station_bounds *d_out_bounds, void *stream, pqp_stats *stats) {
+    if (!h || batch < 0 || total_points < 0 || n_param_sets < 0 || form_mask < 0 || form_mask > 7 ||
+        (batch > 0 && (!d_n_points || !d_offsets || !d_ref || !d_formulation || !d_x0 || !d_end_heading ||
+                       !d_out_states || !d_out_n || !d_out_ok || !d_status)) ||
+        !plan_device_args_ok(bounds_mode, output_mode, batch, d_knot_offsets, d_knots, d_x_coef, d_y_coef,
+                             output_spacing, max_out)) {
+        pqp_set_err("pqp_plan_batch_device_forms: bad argument");
+        return PQP_ERR_ARG;
+    }
+    return plan_batch_device(h, PQP_FORM_KP, form_mask ? form_mask : 7, d_formulation, bounds_mode, output_mode, batch,
+                             total_points, max_n_points, n_param_sets, d_n_points, d_offsets, d_ref, d_map_index,
+                             d_param_index, d_knot_offsets, d_knots, d_x_coef, d_y_coef, d_x0, d_end_heading,
+                             output_spacing, collision_check, max_out, d_out_states, d_out_n, d_out_ok, d_status,
+                             d_iters, d_out_bounds, stream, stats);
 }
 
 int pqp_plan_batch_device(pqp_handle *h, int formulation, int bounds_mode, int output_mode, int batch, int total_points,

@@ -48,6 +48,7 @@ struct pqp_handle {
         int skip = 0, form = 0, n_sets = 1, n_reject = 0;
         cudaStream_t stream = nullptr;
         std::vector<int32_t> n, keep, set;   // (set: empty without a set index)
+        std::vector<int32_t> forms;          // formulation of every path (empty without a per-path formulation)
         std::vector<int> count, start;
         std::vector<size_t> smem;
     } plan;
@@ -67,15 +68,21 @@ struct pqp_handle {
     // allocated until pqp_destroy: a graph captured before the growth still reads it.
     int32_t *d_set_order = nullptr, *d_set_hist = nullptr;
     int set_cap = 0;
+    // device dispatch over per-path formulations (the _forms entries): per-(set, class) order segments over every
+    // formulation's classes (form_cap x all classes x max_batch) and, with a set index, the (set, class, length)
+    // histogram (form_cap x all classes x (largest ncols + 1)); grow-only, outgrown buffers retired as above
+    int32_t *d_form_order = nullptr, *d_form_hist = nullptr;
+    int form_cap = 0;
     std::vector<void *> retired;
     // launches of the last bounds the dispatch was asked for (form, max_n, min_keep, max_keep as passed)
     struct DispatchLaunches {
         bool valid = false;
         int form = 0, max_n = 0, min_keep = 0, max_keep = 0;
+        int max_n_form[3] = {};   // (disp_forms: the bound of every formulation)
         bool reach[PQP_MAX_VARIANTS] = {};
         int min_n[PQP_MAX_VARIANTS] = {};
         size_t smem[PQP_MAX_VARIANTS] = {};
-    } disp;
+    } disp, disp_forms;   // disp_forms: the _forms entries, `form` holding their formulation mask
     // device buffers for the host-pointer entry point
     int32_t *d_n = nullptr, *d_off = nullptr, *d_order = nullptr, *d_status = nullptr, *d_iters = nullptr;
     int32_t *d_order_auto = nullptr;   // launch order computed on the device (pqp_solve_batch_device, small batches)
@@ -100,9 +107,12 @@ struct pqp_handle {
 // pqp_solve_batch_device_classes.
 // `set` [batch]: parameter set of every path (host), NULL: set 0.  A path whose set lies outside the handle's sets is not
 // launched: a small kernel reports it PQP_INVALID_PROBLEM (0 iterations, NaN states).
+// `forms` [batch]: formulation of every path (host), NULL: `form` for every path.  With it each path takes the class of
+// its own formulation (bv.max_k / max_kp set when any path is "KPC"); a path whose formulation is not one of
+// PQP_FORM_* is not launched and reports PQP_INVALID_PROBLEM.
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
                           const pqp_state *ref, const int32_t *keep, cudaStream_t st, int *launches, int form = 0 /* PQP_FORM_KP; 2 = KPC (bv.max_k / max_kp set) */,
-                          const int32_t *set = nullptr);
+                          const int32_t *set = nullptr, const int32_t *forms = nullptr);
 
 // Internal (pqp_capi.cu): the same launches when the station counts exist on the device only.  A dispatch kernel reads
 // them, derives keep_control_steps from the device-side reference states, looks every path up in the class table and
@@ -114,6 +124,16 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
 // lies outside [0, n_sets) reports PQP_INVALID_PROBLEM.
 int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
                         int max_keep, cudaStream_t st, int *launches, const int32_t *d_set = nullptr, int n_param_sets = 0);
+
+// Internal (pqp_capi.cu): pqp_launch_dispatch over per-path formulations.  `d_form` [batch] (device) names every path's
+// formulation; `form_mask` (1 << PQP_FORM_*, nonzero) the ones launched: every (set, class) pair of those formulations
+// the bounds reach.  max_n[f] bounds the paths of formulation f (0: unknown); min_keep / max_keep apply to "KP".  A path
+// whose formulation lies outside the mask, or whose set or length lies outside the bounds, reports
+// PQP_INVALID_PROBLEM.  bv.max_k / max_kp must be set when the mask holds "KPC".  No allocation after a call with the
+// same or a larger set count.
+int pqp_launch_dispatch_forms(pqp_handle *h, const pqp::BatchView &bv, int form_mask, int batch, int total,
+                              const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
+                              const int32_t *d_form, const int32_t *d_set, int n_param_sets);
 
 // thread-local error text returned by pqp_last_error()
 extern thread_local char pqp_g_err[512];

@@ -222,10 +222,13 @@ class PathPlanner(BatchPathSolver):
         map of the set (set_maps) every path is planned on (pqp_plan_batch_maps); None: map 0 (pqp_plan_batch).  A path
         whose index is outside the set reports status -100 (invalid problem), 0 iterations, n_out = 0 and ok = 0.
         `param_index`: int32 [B], the parameter set (set_param_sets) every path is planned with (pqp_plan_batch_sets);
-        None: set 0.  An index outside the sets fails its path the same way."""
-        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
+        None: set 0.  An index outside the sets fails its path the same way.
+        `formulation`: a name for the whole batch, or one per path (pqp_plan_batch_forms): an int32 array [B] of
+        PQP_FORM_* values or a list of names; a value that is not a formulation fails its path the same way."""
         n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
         B = len(n_points)
+        forms = self._forms(formulation, B)
+        form = 0 if forms is not None else FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         ref = np.ascontiguousarray(batch["ref"], dtype=STATE_DTYPE)
         x0 = np.ascontiguousarray(batch["x0"], dtype=np.float64)
         end_heading = np.ascontiguousarray(batch["end_heading"], dtype=np.float64)
@@ -252,7 +255,11 @@ class PathPlanner(BatchPathSolver):
             if mi.shape != (B,) or mi.dtype.kind not in "iu":
                 raise ValueError(f"map_index: expected an integer array of shape ({B},), got {mi.dtype} {mi.shape}")
             mi = np.ascontiguousarray(mi, dtype=np.int32)
-        if param_index is not None:
+        if forms is not None:
+            pi = None if param_index is None else self._param_index(param_index, B)
+            name = "pqp_plan_batch_forms"
+            rc = self._L.pqp_plan_batch_forms(self._h, *head[2:], ptr(mi), ptr(pi), ptr(forms), *tail)
+        elif param_index is not None:
             pi = self._param_index(param_index, B)
             name, rc = "pqp_plan_batch_sets", self._L.pqp_plan_batch_sets(*head, ptr(mi), ptr(pi), *tail)
         elif map_index is None:
@@ -267,7 +274,7 @@ class PathPlanner(BatchPathSolver):
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
                     collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None,
-                    param_index=None, n_param_sets=0):
+                    param_index=None, n_param_sets=0, form_mask=0):
         """plan() on torch CUDA tensors of the planner's device (path_optimizer_b200.device): n_points int32 [B],
         offsets int32 [B + 1], ref float64 [T, 7], x0 float64 [B, 3], end_heading float64 [B]; `splines` (IMPROVED)
         a dict of knot_offsets int32 [B + 1], knots [K], x_coef / y_coef [K, 4] (device.splines_to_device).  The whole
@@ -279,12 +286,16 @@ class PathPlanner(BatchPathSolver):
         as plan(map_index=...)); None: map 0.  A graph replay reads the index from the captured tensor.
         `param_index`: int32 [B] on the device, the parameter set of every path (pqp_plan_batch_device_sets, as
         plan(param_index=...)); None: set 0.  n_param_sets > 0 bounds the sets launched (an index at or past it fails
-        its path).  A graph replays with the sets it was captured with."""
+        its path).  A graph replays with the sets it was captured with.
+        `formulation` one per path (pqp_plan_batch_device_forms): an int32 CUDA tensor [B] of PQP_FORM_* values (a
+        graph replay reads the captured tensor), or an array / list of names, uploaded per call.  `form_mask`
+        (1 << PQP_FORM_* or a list of names; 0: all three) bounds the formulations launched; a path outside it fails."""
         import torch
         from . import device as D
-        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         dev = self._cuda_device()
         B, T = int(n_points.shape[0]), int(ref.shape[0])
+        forms = self._forms_device(formulation, B, dev)
+        form = 0 if forms is not None else FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         f64, i32 = torch.float64, torch.int32
         out = dict(out or {})
         shape = (T, D.STATE_COLS) if output_mode == OUTPUT_RAW else (B, int(max_out), D.STATE_COLS)
@@ -309,7 +320,14 @@ class PathPlanner(BatchPathSolver):
         head = (self._h, form, int(bounds_mode), int(output_mode), B, T, int(max_n_points))
         tail = (float(output_spacing), int(collision_check), int(max_out), *outs,
                 torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
-        if param_index is not None:
+        if forms is not None:
+            mi = D.check(map_index, "map_index", i32, (B,), dev)
+            pi = D.check(param_index, "param_index", i32, (B,), dev)
+            fm = D.check(forms, "formulation", i32, (B,), dev)
+            name = "pqp_plan_batch_device_forms"
+            rc = self._L.pqp_plan_batch_device_forms(self._h, *head[2:], int(n_param_sets), self._form_mask(form_mask),
+                                                     *args[:3], mi, pi, fm, *args[3:], *tail)
+        elif param_index is not None:
             mi = D.check(map_index, "map_index", i32, (B,), dev)
             pi = D.check(param_index, "param_index", i32, (B,), dev)
             name = "pqp_plan_batch_device_sets"

@@ -84,6 +84,43 @@ class BatchPathSolver:
             raise ValueError(f"param_index: expected an integer array of shape ({B},), got {pi.dtype} {pi.shape}")
         return np.ascontiguousarray(pi, dtype=np.int32)
 
+    @staticmethod
+    def _forms(formulation, B):
+        """None for one formulation for the whole batch (a name or an int: today's entries), else the per-path
+        formulations as an int32 numpy array [B] (PQP_FORM_* values; a list of names maps an unknown name to -1, which
+        fails its path).  A torch tensor is returned as it is, for the device entries to check."""
+        if isinstance(formulation, (str, int, np.integer)):
+            return None
+        if type(formulation).__module__.startswith("torch"):
+            return formulation
+        f = list(formulation) if not isinstance(formulation, np.ndarray) else formulation
+        if len(f) and isinstance(f[0], str):
+            f = [FORMULATIONS.get(name, -1) for name in f]
+        f = np.asarray(f)
+        if f.shape != (B,) or f.dtype.kind not in "iu":
+            raise ValueError(f"formulation: expected a name or an integer array / list of names of shape ({B},), "
+                             f"got {f.dtype} {f.shape}")
+        return np.ascontiguousarray(f, dtype=np.int32)
+
+    def _forms_device(self, formulation, B, dev):
+        """The per-path formulations as an int32 CUDA tensor [B] on `dev` (a tensor passes through unchanged, so that a
+        graph replay reads the captured one); None for one formulation for the whole batch."""
+        import torch
+        f = self._forms(formulation, B)
+        if f is None or isinstance(f, torch.Tensor):
+            return f
+        return torch.from_numpy(f).to(dev)
+
+    @staticmethod
+    def _form_mask(form_mask):
+        """An int bitmask (1 << PQP_FORM_*; 0 = all three) or a collection of names / PQP_FORM_* values."""
+        if isinstance(form_mask, (int, np.integer)):
+            return int(form_mask)
+        m = 0
+        for f in form_mask:
+            m |= 1 << (FORMULATIONS[f] if isinstance(f, str) else int(f))
+        return m
+
     def max_points(self, formulation="KP"):
         return self._L.pqp_max_points(self._h, FORMULATIONS[formulation])
 
@@ -92,10 +129,14 @@ class BatchPathSolver:
         status, iters, ok, stats).  `out` may carry preallocated (e.g. pinned) output arrays.
         max_k / max_kp ([sum N] each) are the KPC limits (ReferencePath::getMaxKList / getMaxKpList).
         `param_index`: int32 [B], the parameter set (set_param_sets) every path is solved with (pqp_solve_batch_sets);
-        None: set 0.  A path whose index is outside the sets reports status -100 with 0 iterations and NaN states."""
-        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
+        None: set 0.  A path whose index is outside the sets reports status -100 with 0 iterations and NaN states.
+        `formulation`: a name ("KP", "K", "KPC") for the whole batch, or one per path (pqp_solve_batch_forms): an int32
+        array [B] of PQP_FORM_* values or a list of names.  Path b then gets what a call with its own formulation gives
+        it; a value that is not a formulation fails its path as an out-of-range set index does."""
         n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
         B = len(n_points)
+        forms = self._forms(formulation, B)
+        form = 0 if forms is not None else FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         total = int(n_points.sum())
         ref = np.ascontiguousarray(batch["ref"], dtype=STATE_DTYPE)
         bounds = np.ascontiguousarray(batch["bounds"], dtype=BOUNDS_DTYPE)
@@ -114,7 +155,11 @@ class BatchPathSolver:
             assert len(max_k) == total and len(max_kp) == total
         head = (self._h, form, B, ptr(n_points), ptr(ref), ptr(bounds), ptr(x0), ptr(end_heading), ptr(max_k), ptr(max_kp))
         tail = (ptr(states), ptr(frenet), ptr(status), ptr(iters), C.byref(stats))
-        if param_index is None:
+        if forms is not None:
+            pi = None if param_index is None else self._param_index(param_index, B)
+            name = "pqp_solve_batch_forms"
+            rc = self._L.pqp_solve_batch_forms(self._h, *head[2:], ptr(pi), ptr(forms), *tail)
+        elif param_index is None:
             name, rc = "pqp_solve_batch", self._L.pqp_solve_batch(*head, *tail)
         else:
             pi = self._param_index(param_index, B)
@@ -129,7 +174,7 @@ class BatchPathSolver:
 
     def solve_device(self, n_points, offsets, ref, bounds, x0, end_heading, formulation="KP", max_n_points=0,
                      min_keep=0, max_keep=0, max_k=None, max_kp=None, want_frenet=True, out=None, stats=False,
-                     param_index=None, n_param_sets=0):
+                     param_index=None, n_param_sets=0, form_mask=0):
         """The batch as torch CUDA tensors on the solver's device (path_optimizer_b200.device): n_points int32 [B],
         offsets int32 [B + 1], ref float64 [T, 7], bounds float64 [T, 8], x0 float64 [B, 3], end_heading float64 [B],
         KPC limits float64 [T].  Every path runs on the kernel class solve() would choose for it, picked on the device
@@ -138,12 +183,17 @@ class BatchPathSolver:
         max_n_points / min_keep / max_keep (0 = unknown) only narrow the classes launched; a path outside them reports
         INVALID_PROBLEM.  `out` may carry the output tensors (states, frenet, status, iters).  Returns them as a dict.
         `param_index`: int32 [B] on the device, the parameter set of every path (pqp_solve_batch_device_dispatch_sets);
-        None: set 0.  n_param_sets > 0 bounds the sets launched (an index at or past it reports INVALID_PROBLEM)."""
+        None: set 0.  n_param_sets > 0 bounds the sets launched (an index at or past it reports INVALID_PROBLEM).
+        `formulation` one per path (pqp_solve_batch_device_dispatch_forms): an int32 CUDA tensor [B] of PQP_FORM_*
+        values (a graph replay reads the captured tensor), or an array / list of names, uploaded per call.
+        `form_mask` (1 << PQP_FORM_* or a list of names; 0: all three) bounds the formulations launched; a path outside
+        it reports INVALID_PROBLEM."""
         import torch
         from . import device as D
-        form = FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         dev = self._cuda_device()
         B, T = int(n_points.shape[0]), int(ref.shape[0])
+        forms = self._forms_device(formulation, B, dev)
+        form = 0 if forms is not None else FORMULATIONS[formulation] if isinstance(formulation, str) else int(formulation)
         out = dict(out or {})
         f64, i32 = torch.float64, torch.int32
         states = out.get("states")
@@ -162,7 +212,14 @@ class BatchPathSolver:
         st = Stats()
         tail = (torch.cuda.current_stream(dev).cuda_stream, C.byref(st) if stats else None)
         bounds_ = (self._h, form, B, T, int(max_n_points), int(min_keep), int(max_keep))
-        if param_index is None:
+        if forms is not None:
+            pi = D.check(param_index, "param_index", i32, (B,), dev)
+            fm = D.check(forms, "formulation", i32, (B,), dev)
+            name = "pqp_solve_batch_device_dispatch_forms"
+            rc = self._L.pqp_solve_batch_device_dispatch_forms(self._h, *bounds_[2:], int(n_param_sets),
+                                                               self._form_mask(form_mask), *args[:8], pi, fm, *args[8:],
+                                                               *tail)
+        elif param_index is None:
             name = "pqp_solve_batch_device_dispatch"
             rc = self._L.pqp_solve_batch_device_dispatch(*bounds_, *args, *tail)
         else:
