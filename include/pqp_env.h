@@ -136,6 +136,30 @@ int pqp_update_limits_device(pqp_handle *h, int from_spline, int n, const pqp_st
  * densify tail.  Replaces: tk::spline::set_points. */
 int pqp_spline_fit(int n, const double *t, const double *y, double *coef /* [n][4] */);
 
+/* pqp_spline_fit for every path of a batch on DEVICE arrays of the handle's device: the x(s) and y(s) splines
+ * updateBoundsImproved projects onto (ReferencePathImpl::x_s_, y_s_), in the layout pqp_plan_batch_device* takes with
+ * PQP_BOUNDS_IMPROVED: pass d_offsets as d_knot_offsets and the three outputs as d_knots, d_x_coef, d_y_coef.
+ *   d_offsets          [batch+1] exclusive prefix of the station counts; d_offsets[batch] = total_points
+ *   d_ref              [total_points] reference states; the knots are their s, the values their x and y
+ *   d_knots            [total_points] out: the stations' s, copied as they are
+ *   d_x_coef, d_y_coef [total_points][4] out: pqp_spline_fit's rows for (s, x) and (s, y), bit for bit
+ *   d_ok               [batch] out: 1 when the path was fitted, 0 when it was refused
+ * A path is refused when it has fewer than 3 stations or its s is not strictly increasing or not finite; its knots
+ * and coefficient rows are then NaN, and no other path changes.  (pqp_spline_fit refuses the same paths, except that
+ * it accepts an infinite first or last knot and returns non-finite rows for it.)  To fail a refused path in a plan
+ * call without a host round trip, give it a map index outside the map set on the device, e.g.
+ * map_index[b] = d_ok[b] ? map_index[b] : -1: pqp_plan_batch_device_maps then reports it as PQP_INVALID_PROBLEM with
+ * 0 iterations, out_n = 0 and ok = 0 and no other path changes.
+ * NULL pointers (with batch > 0) or a negative batch or total_points return PQP_ERR_ARG; a batch or total_points
+ * above the handle's capacity PQP_ERR_CAPACITY; nothing is launched then.  Asynchronous on `stream` (NULL: the
+ * handle's stream), no host synchronisation; the scratch (4 doubles per station of the handle's max_total_points) is
+ * allocated by the first call, after which the call allocates nothing and can be captured in a CUDA graph together
+ * with the plan entries.  No map set is needed.
+ * Replaces: tk::spline::set_points through the reference line's (s, x) and (s, y), the splines handed to
+ * ReferencePathImpl::setSpline (reference_path_impl.cpp:36-41), once per path. */
+int pqp_fit_splines_device(pqp_handle *h, int batch, int total_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                           double *d_knots, double *d_x_coef, double *d_y_coef, int32_t *d_ok, void *stream);
+
 /* tk::spline::operator() / deriv (spline.cpp:250-318) on a fitted spline; order 0..2. */
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at);
 

@@ -20,7 +20,7 @@ ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "
                "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device",
                "pqp_set_maps", "pqp_plan_batch_maps", "pqp_plan_batch_device_maps", "pqp_plan_batch_sets",
                "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map",
-               "pqp_plan_batch_forms", "pqp_plan_batch_device_forms"]
+               "pqp_plan_batch_forms", "pqp_plan_batch_device_forms", "pqp_fit_splines_device"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -101,6 +101,7 @@ def load():
     L.pqp_set_maps_occupancy.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap)]
     L.pqp_set_maps_occupancy_device.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap), vp]
     L.pqp_get_map.argtypes = [vp, C.c_int, vp]
+    L.pqp_fit_splines_device.argtypes = [vp, C.c_int, C.c_int] + [vp] * 7
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

@@ -55,6 +55,8 @@ struct EnvState {
     // spline inputs (grow-only): knots + x/y coefficients
     double *d_knots = nullptr, *d_xc = nullptr, *d_yc = nullptr;
     size_t knot_cap = 0;
+    // pqp_fit_splines_device: diag and rhs of both coordinates, 4 doubles per station (max_total, at first use)
+    double *d_fit = nullptr;
     // generic scratch for pqp_map_distance / pqp_check_states (grow-only)
     char *d_tmp = nullptr;
     size_t tmp_cap = 0;
@@ -66,7 +68,7 @@ void env_free(void *p) {
     cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx); cudaFree(e->d_setidx);
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
-    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt);
+    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     delete e;
 }
@@ -363,6 +365,44 @@ pqp_edt_row_kernel(const __grid_constant__ EdtArgs a) {
     const size_t R = (size_t)m.rows, n = R * (size_t)m.cols;
     pqp::edt_row(m.scratch + i, R, m.cols, m.scratch + n + i, m.scratch + 2 * n + i, R, m.res,
                  m.dst + (size_t)i * m.cols);
+}
+
+// pqp_fit_splines_device: one CTA per kFitPaths paths, one thread per (path, coordinate), a path's x and y threads on
+// adjacent lanes.  The CTA first copies the knots of its paths (one range of stations, the offsets being an exclusive
+// prefix), so that no fit reads a knot before it is written; after a barrier every thread decides its path's refusal
+// from the knots, and only after a second barrier may a refused path's x thread overwrite them with NaN.
+constexpr int kFitPaths = 32;
+struct FitArgs {
+    int batch;
+    const int32_t *offsets;
+    const pqp_state *ref;
+    double *knots, *xc, *yc;
+    double *scr;             // 4 doubles per station: diag and rhs of x, then of y
+    int32_t *ok;
+};
+
+__global__ void __launch_bounds__(2 * kFitPaths)
+pqp_fit_splines_kernel(const __grid_constant__ FitArgs a) {
+    const int b0 = blockIdx.x * kFitPaths;
+    const int nb = min(kFitPaths, a.batch - b0);
+    const int lo = a.offsets[b0], hi = a.offsets[b0 + nb];
+    for (int k = lo + (int)threadIdx.x; k < hi; k += blockDim.x) a.knots[k] = a.ref[k].s;
+    __syncthreads();
+    const int p = threadIdx.x >> 1, coord = threadIdx.x & 1;
+    const int b = b0 + p;
+    const bool active = p < nb;
+    int off = 0, n = 0;
+    bool ok = false;
+    if (active) {
+        off = a.offsets[b];
+        n = a.offsets[b + 1] - off;
+        ok = pqp::fit_knots_ok(n, a.knots + off);
+    }
+    __syncthreads();
+    if (!active) return;
+    const size_t o = (size_t)off;
+    pqp::fit_path_coord(max(n, 0), ok, coord, a.ref + o, a.knots + o, (coord ? a.yc : a.xc) + 4 * o, a.scr + 4 * o);
+    if (coord == 0) a.ok[b] = ok ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -787,6 +827,29 @@ int pqp_spline_fit(int n, const double *t, const double *y, double *coef) {
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at) {
     if (n < 1 || !t || !coef || order < 0 || order > 2) return nan("");
     return pqp::spline_eval(SplineView{n, t, coef}, order, at);
+}
+
+int pqp_fit_splines_device(pqp_handle *h, int batch, int total_points, const int32_t *d_offsets, const pqp_state *d_ref,
+                           double *d_knots, double *d_x_coef, double *d_y_coef, int32_t *d_ok, void *stream) {
+    if (!h || batch < 0 || total_points < 0 ||
+        (batch > 0 && (!d_offsets || !d_ref || !d_knots || !d_x_coef || !d_y_coef || !d_ok))) {
+        pqp_set_err("pqp_fit_splines_device: bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (batch > h->max_batch || total_points > h->max_total) {
+        pqp_set_err("batch / total_points exceed what the handle was created for (workspace size)");
+        return PQP_ERR_CAPACITY;
+    }
+    EnvState *e;
+    int rc = env_get(h, &e);
+    if (rc != PQP_OK || batch == 0) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    if (!e->d_fit) PQP_CUDA(cudaMalloc(&e->d_fit, (size_t)h->max_total * 4 * sizeof(double)));
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    const FitArgs a{batch, d_offsets, d_ref, d_knots, d_x_coef, d_y_coef, e->d_fit, d_ok};
+    pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    return PQP_OK;
 }
 
 int pqp_update_bounds_batch(pqp_handle *h, int mode, int batch, const int32_t *n_points, const pqp_state *ref,

@@ -386,6 +386,30 @@ PQP_HD void spline_fit(int n, const double *t, F Y, double *coef, double *diag, 
     coef[4 * (n - 1) + 3] = Y(n - 1);
 }
 
+// The knots pqp_fit_splines_device fits a path's splines on: at least three, finite and strictly increasing.  A strictly
+// increasing sequence lies between its ends, so only the ends need the finiteness test.
+PQP_HD bool fit_knots_ok(int n, const double *t) {
+    return n >= 3 && knots_increasing(n, t) && t[0] >= -1.7976931348623157e308 && t[n - 1] <= 1.7976931348623157e308;
+}
+
+// One thread of pqp_fit_splines_device: coordinate `coord` (0: x, 1: y) of the path whose n stations start at ref,
+// on knots t that are already in place.  coef: that coordinate's n rows; scr: 4n doubles of scratch shared by the
+// path's two threads (x: [0, 2n), y: [2n, 4n)).  A refused path gets NaN rows (the x thread also sets its knots to
+// NaN, so the caller must have finished every read of t by the path's y thread first).
+PQP_HD void fit_path_coord(int n, bool ok, int coord, const pqp_state *ref, double *t, double *coef, double *scr) {
+    static_assert(sizeof(pqp_state) == 7 * sizeof(double), "pqp_state: seven doubles");
+    if (!ok) {
+        const double nan_v = nan("");
+        for (int i = 0; i < 4 * n; ++i) coef[i] = nan_v;
+        if (coord == 0)
+            for (int i = 0; i < n; ++i) t[i] = nan_v;
+        return;
+    }
+    const double *y = coord ? &ref[0].y : &ref[0].x;
+    spline_fit(n, t, [&](int i) { return ldg(y + 7 * (size_t)i); }, coef, scr + 2 * (size_t)coord * n,
+               scr + (2 * (size_t)coord + 1) * n);
+}
+
 // One resampled output state (path_optimizer.cpp:216-222): position from the splines, heading and
 // curvature from their derivatives (getHeading / getCurvature, tools.cpp:34-46).
 PQP_HD pqp_state densify_sample(const SplineView &xs, const SplineView &ys, double ts) {

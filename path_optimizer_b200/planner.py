@@ -271,6 +271,34 @@ class PathPlanner(BatchPathSolver):
         return dict(states=states, n_out=n_out, ok=ok, status=status, iters=iters, bounds=bounds,
                     solved=(status == SOLVED), stats=stats)
 
+    def fit_splines_device(self, offsets, ref, out=None):
+        """reference_splines() on the device (pqp_fit_splines_device): the x(s), y(s) splines of every path of a batch
+        from torch CUDA tensors offsets int32 [B + 1] and ref float64 [T, 7], on torch.cuda.current_stream().  Returns
+        dict(knot_offsets, knots [T], x_coef [T, 4], y_coef [T, 4], ok int32 [B]), ready for plan_device(splines=...):
+        knot_offsets is `offsets` itself, and the coefficients equal spline_fit's bit for bit.  A path with fewer than 3
+        stations or an s that is not finite and strictly increasing gets ok = 0 and NaN knots and rows; fail it in
+        plan_device with map_index = torch.where(ok != 0, map_index, -1).  No host synchronisation; after one warm-up
+        call on the planner it can be captured in a CUDA graph.  `out` may carry the output tensors (knots, x_coef,
+        y_coef, ok), e.g. those of an earlier call, so that a captured graph writes where the plan reads."""
+        import torch
+        from . import device as D
+        dev = self._cuda_device()
+        B, T = int(offsets.shape[0]) - 1, int(ref.shape[0])
+        out = dict(out or {})
+
+        def buf(name, shp, dtype):
+            return out[name] if out.get(name) is not None else torch.empty(shp, dtype=dtype, device=dev)
+        knots, xc, yc = buf("knots", (T,), torch.float64), buf("x_coef", (T, 4), torch.float64), buf("y_coef", (T, 4), torch.float64)
+        ok = buf("ok", (B,), torch.int32)
+        rc = self._L.pqp_fit_splines_device(
+            self._h, B, T, D.check(offsets, "offsets", torch.int32, (B + 1,), dev),
+            D.check(ref, "ref", torch.float64, (T, D.STATE_COLS), dev), D.check(knots, "knots", torch.float64, (T,), dev),
+            D.check(xc, "x_coef", torch.float64, (T, 4), dev), D.check(yc, "y_coef", torch.float64, (T, 4), dev),
+            D.check(ok, "ok", torch.int32, (B,), dev), torch.cuda.current_stream(dev).cuda_stream)
+        if rc != OK:
+            raise PqpError(f"pqp_fit_splines_device failed (rc={rc}): {_lib.last_error()}")
+        return dict(knot_offsets=offsets, knots=knots, x_coef=xc, y_coef=yc, ok=ok)
+
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
                     collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None,
