@@ -82,6 +82,14 @@ struct Kp3 {
     // (only the Ruiz sweeps and diagnostic builds use that row otherwise)
     static constexpr int kExRows = kScratchOnVec ? 7 : 8;
     static constexpr int kCtaScratch = (NW <= 8) ? 128 : 256;   // doubles reserved ahead of the layout for the CTA reductions (16 per warp)
+#ifdef PQP_PHASE_TIMING
+    static constexpr bool kPhTime = !kScratchOnVec;   // (diagnostic builds: which classes record phase times)
+#endif
+    // The 100-station class (config 2's kernel) runs a leaner ADMM iteration: four CTA barriers instead of six (the row
+    // warps of (b2) do not wait for the separator rhs, x-tilde is published without a barrier of its own) and a smaller
+    // inner loop (direct barriers, a rolled held-control loop, no integer division).  Same floating-point operations in
+    // the same order, so the same bits; every other class compiles exactly as before.
+    static constexpr bool kLean = IMAX == 17 && BW == 6 && NW == 4 && MMAX == 17 && FORM == 0;
 
     PQP_HD static Kp3Dims dims(int N, int keep) {
         Kp3Dims d = kp3_dims_raw(N, keep, MMAX);
@@ -105,6 +113,9 @@ struct Kp3 {
         PQP_DEV double *ex(int k) const { return base + 2 * nv + k * kT; }  // 6 exchange rows of kT
         PQP_DEV double *dsS() const { return ex(6); }                     // ds per station     [kT]
         PQP_DEV double *gS() const { return ex(kScratchOnVec ? 5 : 7); }     // separator rhs      [nS <= kT]
+        // 100-station class: per thread, i / L and tid / M as ints in exchange row 4 (in that class only the Ruiz sweeps
+        // use the row), read back in every iteration instead of two integer divisions
+        PQP_DEV int *ixS() const { return reinterpret_cast<int *>(ex(4)); }
         // State only a few threads touch lives in shared memory instead of in (everybody's) registers: the two end rows of
         // the last station (v, W, window: 6 doubles) and the held controls' (v, W, x, sigma), ch each.  It has a region of
         // its own after the exchange rows -- except in the long-path classes, which have no byte to spare: there it sits
@@ -1066,18 +1077,21 @@ struct Kp3 {
             // tasks to the product warps, or two row tasks per loop trip, were slower.)
             const int yT0 = (nSr + 31) & ~31, yNw = kT - yT0;
 #ifdef PQP_PHASE_TIMING
-            static_assert(!kScratchOnVec, "phase timing uses exchange row 5, which the long-path classes give to the separator rhs");
             // clock64() at the phase boundaries, accumulated per warp-0 / warp-1 lead thread in shared scratch
-            // (diagnostic builds only): slots 0..5 = a1, a2, b1, b2, b3, c ; 6 = iterations
+            // (diagnostic builds only): slots 0..5 = a1, a2, b1, b2, b3, c ; 6 = iterations.  Not in the long-path
+            // classes: they give exchange row 5 to the separator rhs.
             double *ph_acc = s.ex(5) + 8 * (wid & 1);   // (row 5 is free once the scaling is done)
-            if ((tid & 31) == 0 && wid < 2) for (int k = 0; k < 8; ++k) ph_acc[k] = 0.0;
+            if (kPhTime && (tid & 31) == 0 && wid < 2) for (int k = 0; k < 8; ++k) ph_acc[k] = 0.0;
             long long ph_t = 0;
-#define PQP_PH(k) if ((tid & 31) == 0 && wid < 2) { const long long now_ = clock64(); ph_acc[k] += (double)(now_ - ph_t); ph_t = now_; }
-#define PQP_PH_START if ((tid & 31) == 0 && wid < 2) { ph_t = clock64(); ph_acc[6] += 1.0; }
+#define PQP_PH(k) if (kPhTime && (tid & 31) == 0 && wid < 2) { const long long now_ = clock64(); ph_acc[k] += (double)(now_ - ph_t); ph_t = now_; }
+#define PQP_PH_START if (kPhTime && (tid & 31) == 0 && wid < 2) { ph_t = clock64(); ph_acc[6] += 1.0; }
 #else
 #define PQP_PH(k)
 #define PQP_PH_START
 #endif
+            // CTA barrier of the iteration.  The 100-station class calls __syncthreads() directly: c.sync() also serves
+            // one-warp CTAs and tests for them at run time, which puts a branch and a warp sync beside every barrier.
+#define PQP_BAR() do { if constexpr (kLean) c.cs.sync(); else c.sync(); } while (0)
             auto step = [&](auto with_check) {
                 PQP_PH_START
                 // ---- (a) g = W (2 clamp(v) - v) per row; rhs = sigma x + A' g
@@ -1085,7 +1099,7 @@ struct Kp3 {
                 const double gD1 = st.WD1 * (2.0 * st.b1 - st.vD1);
                 const double gD2 = st.WD2 * (2.0 * st.b2 - st.vD2);
                 if (st.live) { s.ex(0)[i] = gD0; s.ex(1)[i] = gD1; s.ex(2)[i] = gD2; }
-                c.sync();
+                PQP_BAR();
                 PQP_PH(0)
                 double tsl = 0.0;   // x-tilde of the slack (decouples exactly)
                 double tskp = 0.0;  // KPC: x-tilde of the rate slack of this thread's held control
@@ -1183,15 +1197,20 @@ struct Kp3 {
                 }
                 if (ub.live) {
                     double acc = PQP_UBSG * PQP_UBX + PQP_UBW * (2.0 * clamp2(PQP_UBV, -kOsqpInfty, kOsqpInfty) - PQP_UBV);
-                    for (int t = ub.t0; t <= ub.t1; ++t) acc += s.dsS()[t] * s.ex(2)[t + 1];
+                    if constexpr (kLean) {
+#pragma unroll 1
+                        for (int t = ub.t0; t <= ub.t1; ++t) acc += s.dsS()[t] * s.ex(2)[t + 1];
+                    } else {
+                        for (int t = ub.t0; t <= ub.t1; ++t) acc += s.dsS()[t] * s.ex(2)[t + 1];
+                    }
                     s.tr()[ub.pos] = acc;
                 }
                 }
-                c.sync();
+                PQP_BAR();
                 PQP_PH(1)
                 // ---- (b1) separator rhs g = r_S - T' r_I  (threads 0..3M-1; p fastest -> unit stride, conflict-free)
                 if (tid < nS) {
-                    const int r = tid / M, p = tid - r * M;
+                    const int r = kLean ? s.ixS()[kT + tid] : tid / M, p = tid - r * M;
                     const double *rI = s.tr() + p * d.CS + 3;
                     const double *Tl = s.T() + r * s.nv + p * d.CS + 3;
                     double a0 = rI[r - 3], a1 = 0.0, a2 = 0.0, a3 = 0.0;
@@ -1211,7 +1230,16 @@ struct Kp3 {
                     }
                     s.gS()[3 * p + r] = (a0 + a1) + (a2 + a3);
                 }
-                c.sync();
+                // 100-station class: only the separator product of (b2), on warps 0 and 1 (3M <= 51 threads), reads g_S,
+                // so only those two warps wait for it (named barrier 1, 64 threads).  The row warps go straight on to
+                // y = K_I^-1 r_I, which needs nothing but the rhs.  (The CPU emulator has no partial barrier: full one.)
+#ifndef PQP_HOST_EMU
+                if constexpr (kLean) {
+                    static_assert(!kLean || 3 * MMAX <= 64, "the separator threads fit in warps 0 and 1");
+                    if (wid < 2) asm volatile("bar.sync 1, 64;" ::: "memory");
+                } else
+#endif
+                PQP_BAR();
                 PQP_PH(2)
                 if constexpr (kTwoLevel) {
                     // ---- (b1') reduced right-hand side of the even separators: g'_p = g_p - PL_p g_{p-1} - PR_p g_{p+1}
@@ -1224,7 +1252,7 @@ struct Kp3 {
                         if (pe + 1 < M) a -= lvp[18 + 3 * r] * gS[3 * pe + 3] + lvp[19 + 3 * r] * gS[3 * pe + 4] + lvp[20 + 3 * r] * gS[3 * pe + 5];
                         s.ex(4)[tid] = a;
                     }
-                    c.sync();
+                    PQP_BAR();
                 }
                 // ---- (b2) x_S = Sinv g on the first threads  ||  y = K_I^-1 r_I:
                 //      dense interiors: row tasks (p, k) spread over all the OTHER threads of the CTA;
@@ -1262,7 +1290,7 @@ struct Kp3 {
                         s.ex(3)[xo] = (a0 + a1) + a2;
                     }
                 }
-                c.sync();
+                PQP_BAR();
                 PQP_PH(3)
                 if constexpr (kTwoLevel) {
                     // ---- (b2') odd separators: x_p = E_p (g_p - Off_{p-1}' x_{p-1} - Off_p x_{p+1})  (even entries are read,
@@ -1287,14 +1315,14 @@ struct Kp3 {
                         }
                         s.ex(3)[3 * po + r] = E[3 * r] * t0 + E[3 * r + 1] * t1 + E[3 * r + 2] * t2;
                     }
-                    c.sync();
+                    PQP_BAR();
                 }
                 // ---- (b3) x-tilde: separators take x_S, interiors y - T [x_Sp ; x_Sq]
                 double ta = 0, tb = 0, tc = 0, tu = 0;
 #define PQP_TX(q) ((s.yv()[q] - (Tq[q] * xl0 + Tq[nvs + (q)] * xl1 + Tq[2 * nvs + (q)] * xl2)) \
                    - (Tq[3 * nvs + (q)] * xr0 + Tq[4 * nvs + (q)] * xr1 + Tq[5 * nvs + (q)] * xr2))
                 if (st.live) {
-                    const int p = i / L;
+                    const int p = kLean ? s.ixS()[tid] : i / L;
                     if (st.sep) {
                         ta = s.ex(3)[3 * p]; tb = s.ex(3)[3 * p + 1]; tc = s.ex(3)[3 * p + 2];
                     } else {
@@ -1316,11 +1344,12 @@ struct Kp3 {
                     tu = PQP_TX(ub.pos);
                 }
 #undef PQP_TX
-                // (publishing x-tilde into a vector of its own saves this barrier but was SLOWER)
-                c.sync();   // everyone has consumed tr (rhs): publish x-tilde there for the neighbours
+                // publish x-tilde in tr for the neighbours.  The rhs it overwrites is last read in (b2), before the barrier
+                // that ends it, so the 100-station class publishes at once; the other classes keep their barrier here.
+                if constexpr (!kLean) PQP_BAR();
                 if (st.live) { s.tr()[st.pos] = ta; s.tr()[st.pos + 1] = tb; s.tr()[st.pos + 2] = tc; }
                 if (ub.live) s.tr()[ub.pos] = tu;
-                c.sync();
+                PQP_BAR();
                 PQP_PH(4)
                 // ---- (c) v += alpha (A xt - clamp(v)),  x = alpha xt + (1 - alpha) x
                 if (st.live) {
@@ -1753,6 +1782,7 @@ struct Kp3 {
 #endif
                 }
             };
+#undef PQP_BAR
             // first iteration after `it` that needs the checked form
             auto next_event = [&](int it) {
                 int k = pm.max_iter;
@@ -1763,6 +1793,7 @@ struct Kp3 {
                 }
                 return k;
             };
+            if constexpr (kLean) { s.ixS()[tid] = i / L; s.ixS()[kT + tid] = tid / M; }   // (each thread reads back its own)
             iter = 1;
             while (status == PQP_UNSOLVED && iter < pm.max_iter) {
                 const int ev = next_event(iter);
@@ -1778,7 +1809,7 @@ struct Kp3 {
             if (status == PQP_UNSOLVED) status = PQP_SOLVED_INACCURATE;
         }
 #ifdef PQP_PHASE_TIMING
-        if (bv.debug && (tid & 31) == 0 && wid < 2 && status != PQP_INVALID_PROBLEM) {
+        if (kPhTime && bv.debug && (tid & 31) == 0 && wid < 2 && status != PQP_INVALID_PROBLEM) {
             const double *acc = s.ex(5) + 8 * (wid & 1);
             for (int k = 0; k < 7; ++k) bv.debug[(2 * (size_t)prob + wid) * 8 + k] = (long long)acc[k];
             bv.debug[(2 * (size_t)prob + wid) * 8 + 7] = clock64() - ph_kernel_t0;
