@@ -115,6 +115,11 @@ enum pqp_status {
     PQP_UNSOLVED               = -10,
     PQP_INVALID_PROBLEM        = -100  /* osqp_setup would have refused: l > u, n < 2, ... */
 };
+/* Open corridor sides.  A circle bound of +-1e30 (OSQP_INFTY) or beyond is accepted on a box row.  On the open side of
+ * ONE row of a slack pair (KP: c1_lb or c3_lb opened below, c1_ub or c3_ub above; K: c1; KPC: c2) it makes that row free
+ * while its partner is not: OSQP would weigh the two rows differently (RHO_MIN against rho), and the thread-per-station
+ * kernels, which eliminate the slack on the premise of equal weights, refuse such a path with PQP_INVALID_PROBLEM
+ * (0 iterations, NaN output).  Both rows of a pair opened together are solved. */
 /* Station spacing.  The stations' s need not be evenly spaced; these are refused with PQP_INVALID_PROBLEM (0 iterations,
  * NaN output):
  *  - a NaN or infinite s, in every formulation.  This is a stated rule: the reference would hand the resulting NaN /

@@ -360,31 +360,37 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         const double alpha = pm.alpha;
         double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
         double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;   // primal-infeasibility certificate of the last check
-        iter = 1;
+        iter = 0;
         while (status == PQP_UNSOLVED && iter < pm.max_iter) {
             ++iter;
-            // g_r = W (2 clamp(v) - v) parked in tmp-sized? no: m may exceed n -> reuse E? E is needed.
-            // rhs_j = sigma_j x_j + sum_{r in col j} a_rj W_r (2 clamp(v_r) - v_r), gathered per column
-            for (int j = lane; j < n; j += 32) {
-                double acc = cx.sg[j] * cx.xr[j];
-                for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
-                    const int r = cx.csc_row[e];
-                    const double vv = cx.v[r];
-                    acc += cx.csc_val[e] * (cx.W[r] * (2.0 * clampd(vv, cx.l[r], cx.u[r]) - vv));
-                }
-                cx.tr[j] = acc;
-            }
-            w.sync();
-            gen_solve(w, cx);
             // iterations that end in a termination check first park w = v - clamp(v): the check needs
             // delta_y = W (w_new - w_old) (OSQP update_y / is_primal_infeasible)
             const bool chk = (pm.check_termination && (iter % pm.check_termination == 0)) || iter == pm.max_iter;
-            for (int r = lane; r < m; r += 32) {
-                const double vv = cx.v[r], zz = clampd(vv, cx.l[r], cx.u[r]);
-                if (chk) cx.wold[r] = vv - zz;
-                cx.v[r] = vv + alpha * (gen_row_dot(cx, r, cx.tr) - zz);
+            if (iter == 1) {
+                // OSQP's first iteration from x = z = y = 0 ends at the cold start (x = 0, v = 0: z = clamp(0),
+                // y = -rho clamp(0)).  Its check and rho adaptation still run below, on w_old = y_0 / rho = 0.
+                if (chk) for (int r = lane; r < m; r += 32) cx.wold[r] = 0.0;
+            } else {
+                // g_r = W (2 clamp(v) - v) parked in tmp-sized? no: m may exceed n -> reuse E? E is needed.
+                // rhs_j = sigma_j x_j + sum_{r in col j} a_rj W_r (2 clamp(v_r) - v_r), gathered per column
+                for (int j = lane; j < n; j += 32) {
+                    double acc = cx.sg[j] * cx.xr[j];
+                    for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
+                        const int r = cx.csc_row[e];
+                        const double vv = cx.v[r];
+                        acc += cx.csc_val[e] * (cx.W[r] * (2.0 * clampd(vv, cx.l[r], cx.u[r]) - vv));
+                    }
+                    cx.tr[j] = acc;
+                }
+                w.sync();
+                gen_solve(w, cx);
+                for (int r = lane; r < m; r += 32) {
+                    const double vv = cx.v[r], zz = clampd(vv, cx.l[r], cx.u[r]);
+                    if (chk) cx.wold[r] = vv - zz;
+                    cx.v[r] = vv + alpha * (gen_row_dot(cx, r, cx.tr) - zz);
+                }
+                for (int j = lane; j < n; j += 32) cx.xr[j] = alpha * cx.tr[j] + (1.0 - alpha) * cx.xr[j];
             }
-            for (int j = lane; j < n; j += 32) cx.xr[j] = alpha * cx.tr[j] + (1.0 - alpha) * cx.xr[j];
             w.sync();
             const bool can_check = pm.check_termination && (iter % pm.check_termination == 0);
             const bool can_adapt = pm.adaptive_rho && pm.adaptive_rho_interval && (iter % pm.adaptive_rho_interval == 0);

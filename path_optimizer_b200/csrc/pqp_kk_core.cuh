@@ -903,51 +903,66 @@ struct Kk {
                 else solve_cr(r);
             };
 
-            if (!factor()) status = PQP_NON_CVX;
+            // a +-OSQP_INFTY bound on the open side of one row of the c1 slack pair (rows 9, 10) makes that row free
+            // (RHO_MIN) while its partner keeps the inequality rho; the slack's pivot assumes equal weights: refused
+            // (PQP_INVALID_PROBLEM, 0 iterations; see pqp.h)
+            const bool split = live && rho_bar(E[9] * lo[9], E[9] * hi[9], 1.0) != rho_bar(E[10] * lo[10], E[10] * hi[10], 1.0);
+            if (c.any(split)) status = PQP_INVALID_PROBLEM;
+            else if (!factor()) status = PQP_NON_CVX;
             const double alpha = pm.alpha;
             double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
             double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;
-            iter = 1;
+            iter = 0;
             // (iter % interval == 0 without a division per iteration: the next multiple is tracked)
             const int ct = pm.check_termination, ai = (pm.adaptive_rho ? pm.adaptive_rho_interval : 0);
-            int next_chk = ct == 1 ? 2 : ct, next_ad = ai == 1 ? 2 : ai;
+            int next_chk = ct, next_ad = ai;
             while (status == PQP_UNSOLVED && iter < pm.max_iter) {
                 ++iter;
                 const bool can_check = ct > 0 && iter == next_chk;
                 const bool can_adapt = ai > 0 && iter == next_ad;
                 if (can_check) next_chk += ct;
                 if (can_adapt) next_ad += ai;
-                // rhs = sigma x + A' W (2 clamp(v) - v)
-                double z[11], g[11];
-#pragma unroll
-                for (int k = 0; k < 11; ++k) {
-                    z[k] = clamp2(v[k], lo[k], hi[k]);
-                    g[k] = W[k] * (2.0 * z[k] - v[k]);
-                }
-                if (live) { s.gr(0)[i] = g[0]; s.gr(1)[i] = g[1]; }
-                c.sync();
-                double r[4] = {0, 0, 0, 0}, xt[4] = {0, 0, 0, 0};
-                if (live) {
-                    cols_of(g, r);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) r[q] += sg[q] * x[q];
-                    if (!hasd) r[2] = 0.0;
-                }
-                xt[3] = r[3] * inv_e;
-                kkt_solve(r);
-                xt[0] = r[0]; xt[1] = r[1]; xt[2] = r[2];
                 const bool chk = can_check || iter == pm.max_iter;
-                if (live) {
-                    double ax[11];
-                    rows_of(xt[0], xt[1], xt[2], xt[3], ax);
+                double z[11];
+                if (iter == 1) {
+                    // OSQP's first iteration from x = z = y = 0 ends at the cold start (x = 0, v = 0: z = clamp(0),
+                    // y = -rho clamp(0)).  Its check and rho adaptation still run below, on w_old = y_0 / rho = 0.
+                    if (chk && live) {
+#pragma unroll
+                        for (int k = 0; k < 11; ++k) Wk(k)[tid] = 0.0;
+                    }
+                } else {
+                    // rhs = sigma x + A' W (2 clamp(v) - v)
+                    double g[11];
 #pragma unroll
                     for (int k = 0; k < 11; ++k) {
-                        if (chk) Wk(k)[tid] = v[k] - z[k];
-                        v[k] = v[k] + alpha * (ax[k] - z[k]);
+                        z[k] = clamp2(v[k], lo[k], hi[k]);
+                        g[k] = W[k] * (2.0 * z[k] - v[k]);
                     }
-                    if (last) v[4] = 0.0;
+                    if (live) { s.gr(0)[i] = g[0]; s.gr(1)[i] = g[1]; }
+                    c.sync();
+                    double r[4] = {0, 0, 0, 0}, xt[4] = {0, 0, 0, 0};
+                    if (live) {
+                        cols_of(g, r);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) x[q] = alpha * xt[q] + (1.0 - alpha) * x[q];
+                        for (int q = 0; q < 4; ++q) r[q] += sg[q] * x[q];
+                        if (!hasd) r[2] = 0.0;
+                    }
+                    xt[3] = r[3] * inv_e;
+                    kkt_solve(r);
+                    xt[0] = r[0]; xt[1] = r[1]; xt[2] = r[2];
+                    if (live) {
+                        double ax[11];
+                        rows_of(xt[0], xt[1], xt[2], xt[3], ax);
+#pragma unroll
+                        for (int k = 0; k < 11; ++k) {
+                            if (chk) Wk(k)[tid] = v[k] - z[k];
+                            v[k] = v[k] + alpha * (ax[k] - z[k]);
+                        }
+                        if (last) v[4] = 0.0;
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) x[q] = alpha * xt[q] + (1.0 - alpha) * x[q];
+                    }
                 }
                 if (can_check || can_adapt || iter == pm.max_iter) {
                     c.sync();                        // everybody is done with the x-tilde rows

@@ -805,118 +805,132 @@ PQP_DEV void kp_solve_path(Warp &w, const DevParams &prm, const BatchView &bv, i
         if (lane == 0) s.vEnd()[0] = s.vEnd()[1] = 0.0;
         cx.rho = fmin(fmax(pm.rho, kRhoMin), kRhoMax);
         w.sync();
-        if (!kp_factor(w, cx)) status = PQP_NON_CVX;
+        // a slack pair whose rows fall in different rho classes is refused (see pqp_kp_core3.cuh, pqp.h)
+        int split = 0;
+        for (int i = lane; i < N; i += 32)
+            if (kp_w_box(s.ES4()[i], -kOsqpInfty, s.uS4m()[i], 1.0) != kp_w_box(s.ES4()[i], s.lS4p()[i], kOsqpInfty, 1.0) ||
+                kp_w_box(s.ES2()[i], -kOsqpInfty, s.uS2m()[i], 1.0) != kp_w_box(s.ES2()[i], s.lS2p()[i], kOsqpInfty, 1.0))
+                split = 1;
+        if (w.any(split)) status = PQP_INVALID_PROBLEM;
+        else if (!kp_factor(w, cx)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
         double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
         double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;   // primal-infeasibility certificate of the last check
         // (without a workspace -- test harnesses of this core alone -- infeasibility is not detected)
         double *wold = bv.workspace ? kp_ws_wold(kp_ws_base(bv.workspace, off, prob), N) : nullptr;
-        iter = 1;
+        iter = 0;
         while (status == PQP_UNSOLVED && iter < pm.max_iter) {
             ++iter;
             const double rho = cx.rho;
-            // ---- (a) rhs = sigma_v x + A' W (2 clamp(v) - v)
-            for (int i = lane; i < N; i += 32) {
-                const KpRowW W = kp_row_weights(cx, i, rho);
-                double b0, b1, b2;
-                kp_dyn_bounds(cx, i, b0, b1, b2);
-                s.gD()[i] = W.D0 * (2.0 * b0 - s.vD()[i]);
-                s.gD()[N + i] = W.D1 * (2.0 * b1 - s.vD()[N + i]);
-                s.gD()[2 * N + i] = W.D2 * (2.0 * b2 - s.vD()[2 * N + i]);
-            }
-            w.sync();
-            for (int i = lane; i < N; i += 32) {
-                const KpRowW W = kp_row_weights(cx, i, rho);
-                KpRows g;
-                g.D0 = s.gD()[i]; g.D1 = s.gD()[N + i]; g.D2 = s.gD()[2 * N + i];
-                double v;
-                v = s.vKB()[i]; g.KB = W.KB * (2.0 * clampd(v, -pm.kmax, pm.kmax) - v);
-                v = s.vSB()[i]; g.SB = W.SB * (2.0 * clampd(v, 0.0, pm.margin) - v);
-                v = s.vH1()[i]; g.H1 = W.H1 * (2.0 * clampd(v, s.lH1()[i], s.uH1()[i]) - v);
-                v = s.vH3()[i]; g.H3 = W.H3 * (2.0 * clampd(v, s.lH3()[i], s.uH3()[i]) - v);
-                v = s.vS4m()[i]; g.S4m = W.S4 * (2.0 * clampd(v, -kOsqpInfty, s.uS4m()[i]) - v);
-                v = s.vS4p()[i]; g.S4p = W.S4 * (2.0 * clampd(v, s.lS4p()[i], kOsqpInfty) - v);
-                v = s.vS2m()[i]; g.S2m = W.S2 * (2.0 * clampd(v, -kOsqpInfty, s.uS2m()[i]) - v);
-                v = s.vS2p()[i]; g.S2p = W.S2 * (2.0 * clampd(v, s.lS2p()[i], kOsqpInfty) - v);
-                double gEY = 0, gEH = 0;
-                if (i == N - 1) {
-                    v = s.vEnd()[0]; gEY = kp_w_ey(cx, rho) * (2.0 * clampd(v, -1.0, 1.0) - v);
-                    v = s.vEnd()[1]; gEH = kp_w_eh(cx, rho) * (2.0 * clampd(v, cx.lEH, cx.uEH) - v);
-                }
-                double ra, rb, rc, rs;
-                kp_apply_At(cx, i, g, gEY, gEH, ra, rb, rc, rs);
-                const int ga = kp_gx(d, i);
-                s.tr()[ga] = s.sgr()[ga] * s.xr()[ga] + ra;
-                s.tr()[ga + 1] = s.sgr()[ga + 1] * s.xr()[ga + 1] + rb;
-                s.tr()[ga + 2] = s.sgr()[ga + 2] * s.xr()[ga + 2] + rc;
-                s.ts()[i] = s.sgs()[i] * s.xs()[i] + rs;
-            }
-            for (int j = lane; j < ch; j += 32) {
-                const int gu = kp_gu(d, j);
-                const double v = s.vUB()[j];
-                double acc = s.sgr()[gu] * s.xr()[gu] +
-                             kp_w_ub(cx, j, rho) * (2.0 * clampd(v, -kOsqpInfty, kOsqpInfty) - v);
-                int t1 = j * d.keep + d.keep - 1;
-                if (t1 > N - 2) t1 = N - 2;
-                for (int t = j * d.keep; t <= t1; ++t) acc += s.ds()[t] * s.gD()[2 * N + t + 1];
-                s.tr()[gu] = acc;
-            }
-            w.sync();
-            // ---- (b) reduced KKT solve
-            kp_solve(w, cx);
             // iterations that end in a termination check first park w = v - clamp(v): the check needs
             // delta_y = W (w_new - w_old) (OSQP update_y / is_primal_infeasible)
             const bool chk = wold && ((pm.check_termination && (iter % pm.check_termination == 0)) || iter == pm.max_iter);
-            if (chk) {
+            if (iter == 1) {
+                // OSQP's first iteration from x = z = y = 0 ends at the cold start (x = 0, v = 0: z = clamp(0),
+                // y = -rho clamp(0)).  Its check and rho adaptation still run in (d), on w_old = y_0 / rho = 0.
+                if (chk) for (int k = lane; k < 11 * N + 2; k += 32) wold[k] = 0.0;
+                w.sync();
+            } else {
+                // ---- (a) rhs = sigma_v x + A' W (2 clamp(v) - v)
                 for (int i = lane; i < N; i += 32) {
-                    double b0, b1, b2, v;
+                    const KpRowW W = kp_row_weights(cx, i, rho);
+                    double b0, b1, b2;
                     kp_dyn_bounds(cx, i, b0, b1, b2);
-                    double *wo = wold + i;
-                    wo[0] = s.vD()[i] - b0; wo[N] = s.vD()[N + i] - b1; wo[2 * N] = s.vD()[2 * N + i] - b2;
-                    v = s.vKB()[i]; wo[3 * N] = v - clampd(v, -pm.kmax, pm.kmax);
-                    v = s.vSB()[i]; wo[4 * N] = v - clampd(v, 0.0, pm.margin);
-                    v = s.vH1()[i]; wo[5 * N] = v - clampd(v, s.lH1()[i], s.uH1()[i]);
-                    v = s.vH3()[i]; wo[6 * N] = v - clampd(v, s.lH3()[i], s.uH3()[i]);
-                    v = s.vS4m()[i]; wo[7 * N] = v - clampd(v, -kOsqpInfty, s.uS4m()[i]);
-                    v = s.vS4p()[i]; wo[8 * N] = v - clampd(v, s.lS4p()[i], kOsqpInfty);
-                    v = s.vS2m()[i]; wo[9 * N] = v - clampd(v, -kOsqpInfty, s.uS2m()[i]);
-                    v = s.vS2p()[i]; wo[10 * N] = v - clampd(v, s.lS2p()[i], kOsqpInfty);
+                    s.gD()[i] = W.D0 * (2.0 * b0 - s.vD()[i]);
+                    s.gD()[N + i] = W.D1 * (2.0 * b1 - s.vD()[N + i]);
+                    s.gD()[2 * N + i] = W.D2 * (2.0 * b2 - s.vD()[2 * N + i]);
+                }
+                w.sync();
+                for (int i = lane; i < N; i += 32) {
+                    const KpRowW W = kp_row_weights(cx, i, rho);
+                    KpRows g;
+                    g.D0 = s.gD()[i]; g.D1 = s.gD()[N + i]; g.D2 = s.gD()[2 * N + i];
+                    double v;
+                    v = s.vKB()[i]; g.KB = W.KB * (2.0 * clampd(v, -pm.kmax, pm.kmax) - v);
+                    v = s.vSB()[i]; g.SB = W.SB * (2.0 * clampd(v, 0.0, pm.margin) - v);
+                    v = s.vH1()[i]; g.H1 = W.H1 * (2.0 * clampd(v, s.lH1()[i], s.uH1()[i]) - v);
+                    v = s.vH3()[i]; g.H3 = W.H3 * (2.0 * clampd(v, s.lH3()[i], s.uH3()[i]) - v);
+                    v = s.vS4m()[i]; g.S4m = W.S4 * (2.0 * clampd(v, -kOsqpInfty, s.uS4m()[i]) - v);
+                    v = s.vS4p()[i]; g.S4p = W.S4 * (2.0 * clampd(v, s.lS4p()[i], kOsqpInfty) - v);
+                    v = s.vS2m()[i]; g.S2m = W.S2 * (2.0 * clampd(v, -kOsqpInfty, s.uS2m()[i]) - v);
+                    v = s.vS2p()[i]; g.S2p = W.S2 * (2.0 * clampd(v, s.lS2p()[i], kOsqpInfty) - v);
+                    double gEY = 0, gEH = 0;
                     if (i == N - 1) {
-                        v = s.vEnd()[0]; wold[11 * N] = v - clampd(v, -1.0, 1.0);
-                        v = s.vEnd()[1]; wold[11 * N + 1] = v - clampd(v, cx.lEH, cx.uEH);
+                        v = s.vEnd()[0]; gEY = kp_w_ey(cx, rho) * (2.0 * clampd(v, -1.0, 1.0) - v);
+                        v = s.vEnd()[1]; gEH = kp_w_eh(cx, rho) * (2.0 * clampd(v, cx.lEH, cx.uEH) - v);
+                    }
+                    double ra, rb, rc, rs;
+                    kp_apply_At(cx, i, g, gEY, gEH, ra, rb, rc, rs);
+                    const int ga = kp_gx(d, i);
+                    s.tr()[ga] = s.sgr()[ga] * s.xr()[ga] + ra;
+                    s.tr()[ga + 1] = s.sgr()[ga + 1] * s.xr()[ga + 1] + rb;
+                    s.tr()[ga + 2] = s.sgr()[ga + 2] * s.xr()[ga + 2] + rc;
+                    s.ts()[i] = s.sgs()[i] * s.xs()[i] + rs;
+                }
+                for (int j = lane; j < ch; j += 32) {
+                    const int gu = kp_gu(d, j);
+                    const double v = s.vUB()[j];
+                    double acc = s.sgr()[gu] * s.xr()[gu] +
+                                 kp_w_ub(cx, j, rho) * (2.0 * clampd(v, -kOsqpInfty, kOsqpInfty) - v);
+                    int t1 = j * d.keep + d.keep - 1;
+                    if (t1 > N - 2) t1 = N - 2;
+                    for (int t = j * d.keep; t <= t1; ++t) acc += s.ds()[t] * s.gD()[2 * N + t + 1];
+                    s.tr()[gu] = acc;
+                }
+                w.sync();
+                // ---- (b) reduced KKT solve
+                kp_solve(w, cx);
+                if (chk) {
+                    for (int i = lane; i < N; i += 32) {
+                        double b0, b1, b2, v;
+                        kp_dyn_bounds(cx, i, b0, b1, b2);
+                        double *wo = wold + i;
+                        wo[0] = s.vD()[i] - b0; wo[N] = s.vD()[N + i] - b1; wo[2 * N] = s.vD()[2 * N + i] - b2;
+                        v = s.vKB()[i]; wo[3 * N] = v - clampd(v, -pm.kmax, pm.kmax);
+                        v = s.vSB()[i]; wo[4 * N] = v - clampd(v, 0.0, pm.margin);
+                        v = s.vH1()[i]; wo[5 * N] = v - clampd(v, s.lH1()[i], s.uH1()[i]);
+                        v = s.vH3()[i]; wo[6 * N] = v - clampd(v, s.lH3()[i], s.uH3()[i]);
+                        v = s.vS4m()[i]; wo[7 * N] = v - clampd(v, -kOsqpInfty, s.uS4m()[i]);
+                        v = s.vS4p()[i]; wo[8 * N] = v - clampd(v, s.lS4p()[i], kOsqpInfty);
+                        v = s.vS2m()[i]; wo[9 * N] = v - clampd(v, -kOsqpInfty, s.uS2m()[i]);
+                        v = s.vS2p()[i]; wo[10 * N] = v - clampd(v, s.lS2p()[i], kOsqpInfty);
+                        if (i == N - 1) {
+                            v = s.vEnd()[0]; wold[11 * N] = v - clampd(v, -1.0, 1.0);
+                            v = s.vEnd()[1]; wold[11 * N + 1] = v - clampd(v, cx.lEH, cx.uEH);
+                        }
                     }
                 }
-            }
-            // ---- (c) v += alpha (A xt - clamp(v)),  x = alpha xt + (1 - alpha) x
-            for (int i = lane; i < N; i += 32) {
-                const KpRows zt = kp_apply_A(cx, i, s.tr(), s.ts());
-                double b0, b1, b2, v;
-                kp_dyn_bounds(cx, i, b0, b1, b2);
-                s.vD()[i] += alpha * (zt.D0 - b0);
-                s.vD()[N + i] += alpha * (zt.D1 - b1);
-                s.vD()[2 * N + i] += alpha * (zt.D2 - b2);
-                v = s.vKB()[i]; s.vKB()[i] = v + alpha * (zt.KB - clampd(v, -pm.kmax, pm.kmax));
-                v = s.vSB()[i]; s.vSB()[i] = v + alpha * (zt.SB - clampd(v, 0.0, pm.margin));
-                v = s.vH1()[i]; s.vH1()[i] = v + alpha * (zt.H1 - clampd(v, s.lH1()[i], s.uH1()[i]));
-                v = s.vH3()[i]; s.vH3()[i] = v + alpha * (zt.H3 - clampd(v, s.lH3()[i], s.uH3()[i]));
-                v = s.vS4m()[i]; s.vS4m()[i] = v + alpha * (zt.S4m - clampd(v, -kOsqpInfty, s.uS4m()[i]));
-                v = s.vS4p()[i]; s.vS4p()[i] = v + alpha * (zt.S4p - clampd(v, s.lS4p()[i], kOsqpInfty));
-                v = s.vS2m()[i]; s.vS2m()[i] = v + alpha * (zt.S2m - clampd(v, -kOsqpInfty, s.uS2m()[i]));
-                v = s.vS2p()[i]; s.vS2p()[i] = v + alpha * (zt.S2p - clampd(v, s.lS2p()[i], kOsqpInfty));
-                if (i == N - 1) {
-                    const int ga = kp_gx(d, i);
-                    v = s.vEnd()[0]; s.vEnd()[0] = v + alpha * (s.tr()[ga] - clampd(v, -1.0, 1.0));
-                    v = s.vEnd()[1]; s.vEnd()[1] = v + alpha * (s.tr()[ga + 1] - clampd(v, cx.lEH, cx.uEH));
+                // ---- (c) v += alpha (A xt - clamp(v)),  x = alpha xt + (1 - alpha) x
+                for (int i = lane; i < N; i += 32) {
+                    const KpRows zt = kp_apply_A(cx, i, s.tr(), s.ts());
+                    double b0, b1, b2, v;
+                    kp_dyn_bounds(cx, i, b0, b1, b2);
+                    s.vD()[i] += alpha * (zt.D0 - b0);
+                    s.vD()[N + i] += alpha * (zt.D1 - b1);
+                    s.vD()[2 * N + i] += alpha * (zt.D2 - b2);
+                    v = s.vKB()[i]; s.vKB()[i] = v + alpha * (zt.KB - clampd(v, -pm.kmax, pm.kmax));
+                    v = s.vSB()[i]; s.vSB()[i] = v + alpha * (zt.SB - clampd(v, 0.0, pm.margin));
+                    v = s.vH1()[i]; s.vH1()[i] = v + alpha * (zt.H1 - clampd(v, s.lH1()[i], s.uH1()[i]));
+                    v = s.vH3()[i]; s.vH3()[i] = v + alpha * (zt.H3 - clampd(v, s.lH3()[i], s.uH3()[i]));
+                    v = s.vS4m()[i]; s.vS4m()[i] = v + alpha * (zt.S4m - clampd(v, -kOsqpInfty, s.uS4m()[i]));
+                    v = s.vS4p()[i]; s.vS4p()[i] = v + alpha * (zt.S4p - clampd(v, s.lS4p()[i], kOsqpInfty));
+                    v = s.vS2m()[i]; s.vS2m()[i] = v + alpha * (zt.S2m - clampd(v, -kOsqpInfty, s.uS2m()[i]));
+                    v = s.vS2p()[i]; s.vS2p()[i] = v + alpha * (zt.S2p - clampd(v, s.lS2p()[i], kOsqpInfty));
+                    if (i == N - 1) {
+                        const int ga = kp_gx(d, i);
+                        v = s.vEnd()[0]; s.vEnd()[0] = v + alpha * (s.tr()[ga] - clampd(v, -1.0, 1.0));
+                        v = s.vEnd()[1]; s.vEnd()[1] = v + alpha * (s.tr()[ga + 1] - clampd(v, cx.lEH, cx.uEH));
+                    }
                 }
+                for (int j = lane; j < ch; j += 32) {
+                    const double v = s.vUB()[j];
+                    s.vUB()[j] = v + alpha * (s.tr()[kp_gu(d, j)] - clampd(v, -kOsqpInfty, kOsqpInfty));
+                }
+                w.sync();
+                for (int g = lane; g < d.nred; g += 32) s.xr()[g] = alpha * s.tr()[g] + (1.0 - alpha) * s.xr()[g];
+                for (int i = lane; i < N; i += 32) s.xs()[i] = alpha * s.ts()[i] + (1.0 - alpha) * s.xs()[i];
+                w.sync();
             }
-            for (int j = lane; j < ch; j += 32) {
-                const double v = s.vUB()[j];
-                s.vUB()[j] = v + alpha * (s.tr()[kp_gu(d, j)] - clampd(v, -kOsqpInfty, kOsqpInfty));
-            }
-            w.sync();
-            for (int g = lane; g < d.nred; g += 32) s.xr()[g] = alpha * s.tr()[g] + (1.0 - alpha) * s.xr()[g];
-            for (int i = lane; i < N; i += 32) s.xs()[i] = alpha * s.ts()[i] + (1.0 - alpha) * s.xs()[i];
-            w.sync();
             // ---- (d) residuals, termination, adaptive rho
             const bool can_check = pm.check_termination && (iter % pm.check_termination == 0);
             const bool can_adapt = pm.adaptive_rho && pm.adaptive_rho_interval &&

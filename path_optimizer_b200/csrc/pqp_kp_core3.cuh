@@ -989,18 +989,35 @@ struct Kp3 {
                 return !c.any(!ok);   // (contains CTA barriers)
             };
 
+            // A bound of +-OSQP_INFTY on the open side of a slack-pair row (S4, KP also S2) makes that row free: OSQP gives
+            // it RHO_MIN while its partner keeps the inequality rho.  Unequal weights couple the slack to (a, b), which this
+            // solve relies on not happening: such a path is refused (PQP_INVALID_PROBLEM, 0 iterations; see pqp.h).
+            bool split = false;
+            if (st.live) {
+                const double *w9 = ws + (size_t)kWE * i;
+                split = kp_w_box(w9[7], -kOsqpInfty, st.uS4m, 1.0) != kp_w_box(w9[7], st.lS4p, kOsqpInfty, 1.0);
+                if constexpr (!kKPC)
+                    split = split || kp_w_box(w9[8], -kOsqpInfty, st.uS2m, 1.0) != kp_w_box(w9[8], st.lS2p, kOsqpInfty, 1.0);
+            }
+            if (c.any(split)) status = PQP_INVALID_PROBLEM;
 #ifdef PQP_PHASE_TIMING
             ph_scale = clock64() - ph_scale_t0;
-            { const long long t0_ = clock64(); if (!refactor()) status = PQP_NON_CVX; ph_refactor += clock64() - t0_; }
+            { const long long t0_ = clock64(); if (status == PQP_UNSOLVED && !refactor()) status = PQP_NON_CVX; ph_refactor += clock64() - t0_; }
 #else
-            if (!refactor()) status = PQP_NON_CVX;
+            if (status == PQP_UNSOLVED && !refactor()) status = PQP_NON_CVX;
 #endif
-            const double alpha = pm.alpha;
             const double d1 = pm.d1, d2 = pm.d2, d3 = pm.d3, d4 = pm.d4;
             // An iteration that ends in a termination check needs delta_y = W (w_new - w_old) (OSQP
             // update_y / is_primal_infeasible): w = v - clamp(v) is parked in the workspace at the END
             // of the iteration before it, which keeps the hot part of the loop free of this code.
             auto is_check = [&](int k) { return (pm.check_termination && (k % pm.check_termination == 0)) || k == pm.max_iter; };
+            // OSQP's first iteration from x = z = y = 0 ends at the cold start (x = 0, v = 0: z = clamp(0),
+            // y = -rho clamp(0)).  When it is an event (check, adaptation or the last iteration), it runs as a step
+            // with alpha = 0, which leaves that iterate as it is, followed by (d) on w_old = y_0 / rho = 0.
+            const bool first_event = is_check(1) || (pm.adaptive_rho && pm.adaptive_rho_interval == 1);
+            // (the plain form reads the constant: the inner loop sees no variable alpha)
+            const double alpha_pm = pm.alpha;
+            double alpha_ev = first_event ? 0.0 : alpha_pm;
             auto park_w = [&]() {
                 if constexpr (kKPC) {
                     if (st.live) {
@@ -1093,6 +1110,7 @@ struct Kp3 {
             // one-warp CTAs and tests for them at run time, which puts a branch and a warp sync beside every barrier.
 #define PQP_BAR() do { if constexpr (kLean) c.cs.sync(); else c.sync(); } while (0)
             auto step = [&](auto with_check) {
+                const double alpha = decltype(with_check)::value ? alpha_ev : alpha_pm;
                 PQP_PH_START
                 // ---- (a) g = W (2 clamp(v) - v) per row; rhs = sigma x + A' g
                 const double gD0 = st.WD0 * (2.0 * st.b0 - st.vD0);
@@ -1794,19 +1812,25 @@ struct Kp3 {
                 return k;
             };
             if constexpr (kLean) { s.ixS()[tid] = i / L; s.ixS()[kT + tid] = tid / M; }   // (each thread reads back its own)
-            iter = 1;
+            iter = first_event ? 0 : 1;
+            if (first_event && is_check(1)) {
+                for (int k = tid; k < kWR * N + 2 + (kKPC ? 3 * ch : 0); k += kT) wold[k] = 0.0;
+                c.sync();
+            }
             while (status == PQP_UNSOLVED && iter < pm.max_iter) {
                 const int ev = next_event(iter);
                 while (iter + 1 < ev) {
                     ++iter;
                     step(std::false_type{});
                 }
-                if (is_check(ev)) park_w();
+                if (ev > 1 && is_check(ev)) park_w();
                 ++iter;
                 step(std::true_type{});
+                alpha_ev = alpha_pm;
             }
-            // (max_iter <= 1: the loop never ran; zero residuals pass the 10x check)
+            // (max_iter < 1, which OSQP's settings check refuses: no iteration ran)
             if (status == PQP_UNSOLVED) status = PQP_SOLVED_INACCURATE;
+            if (status == PQP_INVALID_PROBLEM) iter = 0;
         }
 #ifdef PQP_PHASE_TIMING
         if (kPhTime && bv.debug && (tid & 31) == 0 && wid < 2 && status != PQP_INVALID_PROBLEM) {
