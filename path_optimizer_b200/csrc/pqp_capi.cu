@@ -1570,7 +1570,7 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
     }
 #ifdef PQP_PHASE_TIMING
     static long long *d_dbg = nullptr;
-    if (!d_dbg) cudaMalloc(&d_dbg, sizeof(long long) * 32 * 65536);
+    if (!d_dbg) cudaMalloc(&d_dbg, sizeof(long long) * 64 * 65536);
     cudaMemsetAsync(d_dbg, 0, sizeof(long long) * 16 * (size_t)batch, h->stream);
     cudaStreamSynchronize(h->stream);
     bv.debug = d_dbg;
@@ -1697,9 +1697,12 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
         {
             std::vector<long long> g(4 * (size_t)batch);
             cudaMemcpy(g.data(), bv.debug + 16 * 65536, g.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-            double sc = 0, rf = 0, ck = 0, tot = 0, loop = 0;
+            double sc = 0, rf = 0, ck = 0, tot = 0, loop = 0, nref = 0;
+            long long nref_max = 0;
             for (int b = 0; b < batch; ++b) {
                 sc += (double)g[4 * (size_t)b]; rf += (double)g[4 * (size_t)b + 1]; ck += (double)g[4 * (size_t)b + 2];
+                nref += (double)g[4 * (size_t)b + 3];
+                nref_max = std::max(nref_max, g[4 * (size_t)b + 3]);
                 tot += (double)dbg[(2 * (size_t)b) * 8 + 7];
                 for (int k = 0; k < 6; ++k) loop += (double)dbg[(2 * (size_t)b) * 8 + k];
             }
@@ -1709,8 +1712,17 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
             for (int b = 0; b < batch; ++b) for (int k = 0; k < 8; ++k) rt[k] += (double)g2[8 * (size_t)b + k] / batch;
             fprintf(stderr, "[refactor cycles per path, all refactorisations] weights=%.0f assembly=%.0f interior LDL=%.0f spikes=%.0f schur=%.0f block LDL=%.0f dense Sinv=%.0f dense interiors=%.0f\n",
                     rt[0], rt[1], rt[2], rt[3], rt[4], rt[5], rt[6], rt[7]);
-            fprintf(stderr, "[cycles per path] kernel=%.0f  iterations(a..c)=%.0f  scaling=%.0f  refactor(all)=%.0f  check blocks(all, incl. their refactors)=%.0f\n",
+            fprintf(stderr, "[cycles per path] kernel=%.0f  iterations(a..c)=%.0f  scaling=%.0f  refactor(all)=%.0f  check blocks(all, without their refactors)=%.0f\n",
                     tot / batch, loop / batch, sc / batch, rf / batch, ck / batch);
+            fprintf(stderr, "[refactorisations per path] mean=%.2f max=%lld\n", nref / batch, nref_max);
+            std::vector<long long> g3(32 * (size_t)batch);
+            cudaMemcpy(g3.data(), bv.debug + 32 * 65536, g3.size() * sizeof(long long), cudaMemcpyDeviceToHost);
+            for (int w = 0; w < 4; ++w) {
+                double ckp[6] = {0};
+                for (int b = 0; b < batch; ++b) for (int k = 0; k < 6; ++k) ckp[k] += (double)g3[32 * (size_t)b + 8 * w + k] / batch;
+                fprintf(stderr, "[check-block cycles per path, all checks, warp %d] loads+publish x=%.0f primal=%.0f barrier=%.0f dual=%.0f certificate=%.0f reduction=%.0f\n",
+                        w, ckp[0], ckp[1], ckp[2], ckp[3], ckp[4], ckp[5]);
+            }
         }
     }
 #endif

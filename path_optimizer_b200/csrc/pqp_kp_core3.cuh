@@ -211,8 +211,9 @@ struct Kp3 {
         const int lane = c.lane(), tid = c.tid(), wid = c.wid;
 #ifdef PQP_PHASE_TIMING
         const long long ph_kernel_t0 = clock64();
-        long long ph_refactor = 0, ph_check = 0, ph_scale = 0;
+        long long ph_refactor = 0, ph_check = 0, ph_scale = 0, ph_nref = 0;
         long long rt_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, rt_t = 0;
+        long long ck_acc[6] = {0, 0, 0, 0, 0, 0}, ck_t = 0;   // check block (d), per warp: see PQP_CK
 #endif
         const int N = bv.n_points[prob];
         const int off = bv.offsets[prob];
@@ -1002,7 +1003,11 @@ struct Kp3 {
             if (c.any(split)) status = PQP_INVALID_PROBLEM;
 #ifdef PQP_PHASE_TIMING
             ph_scale = clock64() - ph_scale_t0;
-            { const long long t0_ = clock64(); if (status == PQP_UNSOLVED && !refactor()) status = PQP_NON_CVX; ph_refactor += clock64() - t0_; }
+            {
+                const long long t0_ = clock64();
+                if (status == PQP_UNSOLVED) { ++ph_nref; if (!refactor()) status = PQP_NON_CVX; }
+                ph_refactor += clock64() - t0_;
+            }
 #else
             if (status == PQP_UNSOLVED && !refactor()) status = PQP_NON_CVX;
 #endif
@@ -1433,6 +1438,13 @@ struct Kp3 {
                 PQP_PH(5)
                 // ---- (d) residuals, termination, adaptive rho
                 if constexpr (decltype(with_check)::value) {
+#ifdef PQP_PHASE_TIMING
+// lane 0 of every warp: 0 loads + x publish, 1 primal pass, 2 its barrier, 3 dual pass, 4 certificate, 5 reduction
+#define PQP_CK(k) if (lane == 0) { const long long now_ = clock64(); ck_acc[k] += now_ - ck_t; ck_t = now_; }
+                    if (lane == 0) ck_t = clock64();
+#else
+#define PQP_CK(k)
+#endif
                     const bool can_check = pm.check_termination && (iter % pm.check_termination == 0);
                     const bool can_adapt = pm.adaptive_rho && pm.adaptive_rho_interval &&
                                            (iter % pm.adaptive_rho_interval == 0);
@@ -1456,6 +1468,7 @@ struct Kp3 {
                     if (st.live) { s.tr()[st.pos] = st.xa; s.tr()[st.pos + 1] = st.xb; s.tr()[st.pos + 2] = st.xc; }
                     if (ub.live) s.tr()[ub.pos] = PQP_UBX;
                     c.sync();
+                    PQP_CK(0)
                     double pr = 0, nz = 0, nax = 0, prs = 0, nzs = 0, naxs = 0;
                     double dr = 0, npx = 0, naty = 0, drs = 0, npxs = 0, natys = 0;
                     const double cinv = 1.0 / cost_c;
@@ -1529,7 +1542,9 @@ struct Kp3 {
                             PQP_ROW(PQP_UBX, PQP_UBV, -kOsqpInfty, kOsqpInfty, ws[oEU + tid])
                         }
                     }
+                    PQP_CK(1)
                     c.sync();
+                    PQP_CK(2)
                     if constexpr (kKPC) {
                       if (st.live) {
                         const double yKL = PQP_DUAL(st.vKL, -st.mk, kOsqpInfty, st.WK);
@@ -1613,6 +1628,7 @@ struct Kp3 {
                     // ---- primal-infeasibility certificate (OSQP is_primal_infeasible) in unscaled terms:
                     // g = W (w_new - w_old) = E delta_y, projected on the cone of the finite bounds;
                     // ||g||_inf, u'g+ + l'g-, ||A'g||_inf.  The control rows are free (g = 0).
+                    PQP_CK(3)
                     double c_nrm = 0, c_lhs = 0, c_cert = 0;
                     if (chk) {
 #define PQP_G(V, LO, HI, WW, WO) ((WW) * (((V) - clamp2((V), (LO), (HI))) - (WO)))
@@ -1720,15 +1736,45 @@ struct Kp3 {
                         }
 #undef PQP_G
 #undef PQP_ACC
-                        c_lhs = c.sum(c_lhs);
                     }
+                    PQP_CK(4)
                     {
+                        // the 14 maxima and (checks only) the certificate's sum u'g+ + l'g- over the CTA in ONE shared
+                        // exchange: warp butterflies, one slot row of 16 per warp, and the cross-warp combine unrolled
+                        // over the compile-time warp count.  Same operations in the same order as Cta::max_n and
+                        // Cta::sum (warp 0's partial first, then warps 1, 2, ...), so the same bits.
                         double red[14] = {pr, nz, nax, prs, nzs, naxs, dr, npx, naty, drs, npxs, natys, c_nrm, c_cert};
-                        c.max_n(red, 14);
+                        static_assert(NW > 1 && 16 * NW <= kCtaScratch, "one slot row of 16 per warp");
+#pragma unroll
+                        for (int k = 0; k < 14; ++k) red[k] = c.w.max(red[k]);
+                        if (chk) c_lhs = c.w.sum(c_lhs);
+                        double *const sc = c.scratch;
+                        if (lane == 0) {
+#pragma unroll
+                            for (int k = 0; k < 14; ++k) sc[wid * 16 + k] = red[k];
+                            sc[wid * 16 + 14] = c_lhs;
+                        }
+                        c.cs.sync();
+#pragma unroll
+                        for (int k = 0; k < 14; ++k) {
+                            double r = sc[k];
+#pragma unroll
+                            for (int q = 1; q < NW; ++q) r = fmax(r, sc[q * 16 + k]);
+                            red[k] = r;
+                        }
+                        if (chk) {
+                            double r = sc[14];
+#pragma unroll
+                            for (int q = 1; q < NW; ++q) r += sc[q * 16 + 14];
+                            c_lhs = r;
+                        }
+                        c.cs.sync();
                         pr = red[0]; nz = red[1]; nax = red[2]; prs = red[3]; nzs = red[4]; naxs = red[5];
                         dr = red[6]; npx = red[7]; naty = red[8]; drs = red[9]; npxs = red[10]; natys = red[11];
                         c_nrm = red[12]; c_cert = red[13];
                     }
+                    PQP_CK(5)
+#undef PQP_CK
                     // No residual or certificate is carried across iterations (registers): the 10x
                     // re-check OSQP does when max_iter is reached is decided right here.
                     const double pri_res = pr, dua_res = dr;
@@ -1789,14 +1835,19 @@ struct Kp3 {
                             rho = rho_new;
                             c.sync();
 #ifdef PQP_PHASE_TIMING
-                            { const long long t0_ = clock64(); if (!refactor()) status = PQP_NON_CVX; ph_refactor += clock64() - t0_; }
+                            {   // (counted in ph_refactor, not in ph_check)
+                                const long long t0_ = clock64();
+                                if (!refactor()) status = PQP_NON_CVX;
+                                const long long dt_ = clock64() - t0_;
+                                ph_refactor += dt_; ph_check -= dt_; ++ph_nref;
+                            }
 #else
                             if (!refactor()) status = PQP_NON_CVX;
 #endif
                         }
                     }
 #ifdef PQP_PHASE_TIMING
-                    ph_check += clock64() - ph_t;   // (includes a refactorisation when one happened)
+                    ph_check += clock64() - ph_t;   // (a refactorisation it triggered is subtracted above)
 #endif
                 }
             };
@@ -1839,10 +1890,16 @@ struct Kp3 {
             bv.debug[(2 * (size_t)prob + wid) * 8 + 7] = clock64() - ph_kernel_t0;
             if (wid == 0) {
                 long long *g = bv.debug + 16 * 65536 + 4 * (size_t)prob;
-                g[0] = ph_scale; g[1] = ph_refactor; g[2] = ph_check;
+                g[0] = ph_scale; g[1] = ph_refactor; g[2] = ph_check; g[3] = ph_nref;
                 long long *g2 = bv.debug + 20 * 65536 + 8 * (size_t)prob;
                 for (int k = 0; k < 8; ++k) g2[k] = rt_acc[k];
             }
+        }
+#endif
+#ifdef PQP_PHASE_TIMING
+        if (kPhTime && bv.debug && lane == 0 && wid < 4 && status != PQP_INVALID_PROBLEM) {
+            long long *g3 = bv.debug + 32 * 65536 + 32 * (size_t)prob + 8 * wid;
+            for (int k = 0; k < 6; ++k) g3[k] = ck_acc[k];
         }
 #endif
         // ---- epilogue: getOptimizedPath, solver_kp_as_input.cpp:26-43
