@@ -214,26 +214,32 @@ static int launch_variant(pqp_handle *h, int v, const pqp::DevParams *prm, const
                           const int32_t *d_order, size_t smem_bytes, cudaStream_t st);
 }
 
+// What a kernel writes into the stations of a path it cannot take (with PQP_INVALID_PROBLEM and 0 iterations): NaN
+// states, v = a = 0, NaN Frenet states.  Stations i0, i0 + step, ... of the n at `off`.
+__device__ __forceinline__ void write_invalid(pqp_state *out_states, double *out_frenet, int off, int n, int i0,
+                                              int step) {
+    const double qnan = nan("");
+    for (int i = i0; i < n; i += step) {
+        pqp_state &o = out_states[off + i];
+        o.x = o.y = o.z = o.k = o.s = qnan;
+        o.v = o.a = 0.0;
+        if (out_frenet) {
+            double *f = out_frenet + 3 * (size_t)(off + i);
+            f[0] = f[1] = f[2] = qnan;
+        }
+    }
+}
+
 // Paths a host plan does not launch because their parameter set is out of range: one CTA per order entry writes what a
 // kernel writes for a path it cannot take (PQP_INVALID_PROBLEM, 0 iterations, NaN states).
 __global__ void __launch_bounds__(128)
 pqp_reject_kernel(const __grid_constant__ pqp::BatchView bv, const int32_t *__restrict__ order) {
     const int b = order[blockIdx.x];
-    const int n = bv.n_points[b], off = bv.offsets[b];
     if (threadIdx.x == 0) {
         bv.status[b] = PQP_INVALID_PROBLEM;
         if (bv.iters) bv.iters[b] = 0;
     }
-    const double qnan = nan("");
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        pqp_state &o = bv.out_states[off + i];
-        o.x = o.y = o.z = o.k = o.s = qnan;
-        o.v = o.a = 0.0;
-        if (bv.out_frenet) {
-            double *f = bv.out_frenet + 3 * (size_t)(off + i);
-            f[0] = f[1] = f[2] = qnan;
-        }
-    }
+    write_invalid(bv.out_states, bv.out_frenet, bv.offsets[b], bv.n_points[b], threadIdx.x, blockDim.x);
 }
 
 // One launch per (set, class) segment g = set * kNumVariants + v with count[g] > 0: count[g] CTAs over the order entries
@@ -281,6 +287,44 @@ static int launch_class_set(pqp_handle *h, const pqp::BatchView &bv, int n_sets,
     return rc;
 }
 
+// The host class plan of the paths [b0, b1): every path's segment g = set * kNumVariants + class (class_for on its
+// length, keep and formulation; `set` / `forms` NULL: set 0 / `form` for every path), or segment G = n_sets *
+// kNumVariants when its set lies outside [0, n_sets) or its formulation is none (rejected, not launched).  Fills
+// count[0, G], start[0, G + 1] (start[0] = b0), smem[0, G] and h->h_order[b0, b1): the segments in turn, each stably
+// sorted longest EXPECTED WORK first with a hint (pqp_set_order_hint: stations x expected iterations), else by `before`.
+template <class Before>
+static void plan_classes(pqp_handle *h, int batch, int b0, int b1, int n_sets, const int32_t *n, const int32_t *keep,
+                         int form, const int32_t *forms, const int32_t *set, Before before, int *count, int *start,
+                         size_t *smem) {
+    const int G = n_sets * kNumVariants;
+    std::vector<int> seg((size_t)(b1 - b0));
+    std::fill(count, count + G + 1, 0);
+    std::fill(smem, smem + G + 1, 0);
+    for (int b = b0; b < b1; ++b) {
+        const int s = set ? set[b] : 0;
+        const int f = forms ? forms[b] : form;
+        int &g = seg[b - b0];
+        if (s < 0 || s >= n_sets || (forms && !pqp::form_in_mask(f, 7))) { g = G; count[G]++; continue; }
+        int v;
+        size_t need;
+        class_for(h, n[b], keep[b], &v, &need, f);
+        g = s * kNumVariants + v;
+        smem[g] = std::max(smem[g], need);
+        count[g]++;
+    }
+    start[0] = b0;
+    for (int g = 0; g <= G; ++g) start[g + 1] = start[g] + count[g];
+    std::vector<int> fill(start, start + G + 1);
+    for (int b = b0; b < b1; ++b) h->h_order[fill[seg[b - b0]]++] = b;
+    const bool hinted = h->order_hint.size() == (size_t)batch;
+    const int32_t *hint = h->order_hint.data();
+    for (int g = 0; g < G; ++g)
+        std::stable_sort(h->h_order + start[g], h->h_order + start[g + 1], [&](int a, int b) {
+            if (hinted) return (long long)n[a] * hint[a] > (long long)n[b] * hint[b];
+            return before(a, b);
+        });
+}
+
 int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, const int32_t *n, const int32_t *off,
                           const pqp_state *ref, const int32_t *keep_in, cudaStream_t st, int *launches, int form,
                           const int32_t *set, const int32_t *forms) {
@@ -292,6 +336,7 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
         keepv[b] = f == PQP_FORM_KPC ? 4 : f == PQP_FORM_K ? 1 : keep_in ? keep_in[b] : (n[b] >= 2 ? pqp_keep_control_steps(PQP_FORM_KP, ref + off[b], n[b]) : 1);
     }
     const int n_sets = set ? (int)h->dsets.size() : 1;
+    const int G = n_sets * kNumVariants;   // segment G: the rejected paths
     // The plan (segment per path, longest-first order inside a segment) only depends on (n, keep, set, formulation): a
     // caller that solves batches of the same shape back to back reuses it, and the order array already on the device
     // with it.
@@ -305,33 +350,12 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
         PQP_CUDA(cudaStreamSynchronize(st));
         if (pl.stream && pl.stream != st) PQP_CUDA(cudaStreamSynchronize(pl.stream));
         pl.valid = false;
-        const int G = n_sets * kNumVariants;   // segment G: the rejected paths
-        std::vector<int> seg((size_t)batch);
-        pl.count.assign((size_t)G + 1, 0);
-        pl.start.assign((size_t)G + 2, 0);
-        pl.smem.assign((size_t)G + 1, 0);
-        for (int b = 0; b < batch; ++b) {
-            const int s = set ? set[b] : 0;
-            const int f = forms ? forms[b] : form;
-            if (s < 0 || s >= n_sets || (forms && !pqp::form_in_mask(f, 7))) { seg[b] = G; pl.count[G]++; continue; }
-            int v;
-            size_t need;
-            class_for(h, n[b], keepv[b], &v, &need, f);
-            seg[b] = s * kNumVariants + v;
-            pl.smem[seg[b]] = std::max(pl.smem[seg[b]], need);
-            pl.count[seg[b]]++;
-        }
-        for (int g = 0; g <= G; ++g) pl.start[g + 1] = pl.start[g] + pl.count[g];
-        std::vector<int> fill(pl.start.begin(), pl.start.end() - 1);
-        for (int b = 0; b < batch; ++b) h->h_order[fill[seg[b]]++] = b;
-        // longest first; with a hint (pqp_set_order_hint) longest EXPECTED WORK first: stations x expected iterations
-        const bool hinted = h->order_hint.size() == (size_t)batch;
-        const int32_t *hint = h->order_hint.data();
-        for (int g = 0; g < G; ++g)
-            std::stable_sort(h->h_order + pl.start[g], h->h_order + pl.start[g + 1], [&](int a, int b) {
-                if (hinted) return (long long)n[a] * hint[a] > (long long)n[b] * hint[b];
-                return n[a] > n[b];
-            });
+        pl.count.resize((size_t)G + 1);
+        pl.start.resize((size_t)G + 2);
+        pl.smem.resize((size_t)G + 1);
+        auto longest = [&](int a, int b) { return n[a] > n[b]; };
+        plan_classes(h, batch, 0, batch, n_sets, n, keepv.data(), form, forms, set, longest, pl.count.data(),
+                     pl.start.data(), pl.smem.data());
         PQP_CUDA(cudaMemcpyAsync(h->d_order, h->h_order, (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
         pl.n.assign(n, n + batch);
         pl.keep = keepv;
@@ -340,15 +364,13 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
         if (forms) pl.forms.assign(forms, forms + batch);
         else pl.forms.clear();
         pl.n_sets = n_sets;
-        pl.n_reject = pl.count[G];
         pl.skip = (int)skip_mask();
         pl.form = form;
         pl.stream = st;
         pl.valid = true;
     }
-    const int G = n_sets * kNumVariants;
     return launch_class_set(h, bv, n_sets, pl.count.data(), pl.start.data(), pl.smem.data(), h->d_order, st, launches,
-                            pl.n_reject, pl.start[G]);
+                            pl.count[G], pl.start[G]);
 }
 
 // ---- class selection on the device -------------------------------------------------------------------------------
@@ -364,8 +386,11 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
 // and spills in 11 of the 16 solve kernels, which sit at their register limits.
 constexpr int kDispatchThreads = 1024;
 struct DispatchArgs {
-    const int8_t *table;
-    int ncols, form, v0, nv, max_n, min_keep, max_keep, batch;
+    pqp::FormTables t;         // class table, ncols and length bound of every formulation
+    const int32_t *form_of;    // [batch] formulation of every path, NULL: `form` for every path
+    int form, form_mask;       // the call's single formulation (mask_form(form_mask)) and the formulations launched
+    int v0, nv, ncols;         // order layout: the classes [v0, v0 + nv) the mask spans, `ncols` length buckets each
+    int min_keep, max_keep, batch;
     const int32_t *n_points, *offsets;
     const pqp_state *ref;
     pqp_state *out_states;
@@ -377,37 +402,44 @@ struct DispatchArgs {
     const int32_t *set;        // [batch] parameter set of every path, NULL: set 0
     int n_sets;                // sets launched: a path whose set lies outside [0, n_sets) is answered here; 1 without `set`
     int32_t *hist;             // [n_sets * nv * ncols + n_sets * nv] histogram and bases in global memory, NULL: shared
-    const int32_t *form_of;    // pqp_dispatch_forms_kernel: [batch] formulation of every path
-    int form_mask;             //   and the formulations launched (1 << PQP_FORM_*)
 };
 
 __global__ void pqp_fill_kernel(int32_t *p, size_t n, int32_t value) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = value;
 }
 
-// A path the dispatch does not launch, answered as a kernel answers a path it cannot take.
-__device__ __forceinline__ void dispatch_reject(const DispatchArgs &a, int b, int n, int off) {
-    a.status[b] = PQP_INVALID_PROBLEM;
-    a.iters[b] = 0;
-    const double qnan = nan("");
-    for (int i = 0; i < n; ++i) {
-        pqp_state &o = a.out_states[off + i];
-        o.x = o.y = o.z = o.k = o.s = qnan;
-        o.v = o.a = 0.0;
-        if (a.out_frenet) {
-            double *f = a.out_frenet + 3 * (size_t)(off + i);
-            f[0] = f[1] = f[2] = qnan;
+__global__ void __launch_bounds__(kDispatchThreads)
+pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
+    // [n_sets * nv * ncols] paths per (set, class, longest-first length bucket), then [n_sets * nv] bases: in shared
+    // memory for one set, in global memory (a.hist) for several
+    extern __shared__ int32_t hist_s[];
+    __shared__ int32_t warp_sum[kDispatchThreads / 32];
+    int32_t *hist = a.hist ? a.hist : hist_s;
+    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
+    if (tid == 0) a.n_view[a.batch] = 0;
+    __syncthreads();
+    for (int b = tid; b < a.batch; b += kDispatchThreads) {
+        const int n = a.n_points[b], off = a.offsets[b];
+        a.n_view[b] = n;
+        const int s = a.set ? a.set[b] : 0;
+        const int f = a.form_of ? a.form_of[b] : a.form;
+        const bool ok = pqp::form_in_mask(f, a.form_mask) && s >= 0 && s < a.n_sets;
+        const int keep = ok ? pqp::keep_control_steps(f, a.ref + off, n) : 0;
+        const int key = pqp::dispatch_key_forms(a.t, a.form_mask, f, s, a.n_sets, n, keep, a.min_keep, a.max_keep, a.nv,
+                                                a.ncols, a.v0);
+        if (key >= 0) {
+            atomicAdd(&hist[key], 1);
+        } else {   // not launched: answered as a kernel answers a path it cannot take
+            a.status[b] = PQP_INVALID_PROBLEM;
+            a.iters[b] = 0;
+            write_invalid(a.out_states, a.out_frenet, off, n, 0, 1);
         }
+        a.key[b] = key;
     }
-}
-
-// The second half of both dispatch kernels, once every path's key is in a.key and counted in hist[0, nsv * ncols):
-// exclusive prefix of the histogram, then the scatter into the order segments (nsv of them, `batch` entries each).
-__device__ __forceinline__ void dispatch_scatter(const DispatchArgs &a, int32_t *hist, int nsv, int ncols,
-                                                 int32_t *warp_sum) {
-    const int nb = nsv * ncols, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    int32_t *base = hist + nb;
+    __syncthreads();
     // exclusive prefix of the histogram: every thread owns a run of consecutive buckets
+    int32_t *base = hist + nb;
     const int per = (nb + kDispatchThreads - 1) / kDispatchThreads, lo = min(tid * per, nb), hi = min(lo + per, nb);
     int sum = 0;
     for (int i = lo; i < hi; ++i) sum += hist[i];
@@ -435,78 +467,21 @@ __device__ __forceinline__ void dispatch_scatter(const DispatchArgs &a, int32_t 
         run += c;
     }
     __syncthreads();
-    for (int r = tid; r < nsv; r += kDispatchThreads) base[r] = hist[r * ncols];
+    // scatter into the order segments (nsv of them, `batch` entries each)
+    for (int r = tid; r < nsv; r += kDispatchThreads) base[r] = hist[r * a.ncols];
     __syncthreads();
     for (int b = tid; b < a.batch; b += kDispatchThreads) {
         const int key = a.key[b];
         if (key < 0) continue;
-        const int r = key / ncols;
+        const int r = key / a.ncols;
         a.order[(size_t)r * a.batch + (atomicAdd(&hist[key], 1) - base[r])] = b;
     }
 }
 
-__global__ void __launch_bounds__(kDispatchThreads)
-pqp_dispatch_kernel(const __grid_constant__ DispatchArgs a) {
-    // [n_sets * nv * ncols] paths per (set, class, longest-first length bucket), then [n_sets * nv] bases: in shared
-    // memory for one set, in global memory (a.hist) for several
-    extern __shared__ int32_t hist_s[];
-    __shared__ int32_t warp_sum[kDispatchThreads / 32];
-    int32_t *hist = a.hist ? a.hist : hist_s;
-    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x;
-    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
-    if (tid == 0) a.n_view[a.batch] = 0;
-    __syncthreads();
-    for (int b = tid; b < a.batch; b += kDispatchThreads) {
-        const int n = a.n_points[b], off = a.offsets[b];
-        a.n_view[b] = n;
-        const int s = a.set ? a.set[b] : 0;
-        const bool set_ok = s >= 0 && s < a.n_sets;
-        const int keep = set_ok ? pqp::keep_control_steps(a.form, a.ref + off, n) : 0;
-        const int v = set_ok ? pqp::dispatch_class(a.table, a.ncols, a.form, n, keep, a.max_n, a.min_keep, a.max_keep) : -1;
-        int key = -1;
-        if (v >= 0) {
-            key = pqp::dispatch_key(s, v - a.v0, a.nv, a.ncols, n);
-            atomicAdd(&hist[key], 1);
-        } else {
-            dispatch_reject(a, b, n, off);
-        }
-        a.key[b] = key;
-    }
-    __syncthreads();
-    dispatch_scatter(a, hist, nsv, a.ncols, warp_sum);
-}
-
-// The dispatch over per-path formulations: every path looks its class up in the table of its own formulation
-// (t.table[a.form_of[b]]) and is keyed by (set, class of the whole variant space, length) with
-// pqp::dispatch_key_forms; a.nv = every class, a.ncols = the stride shared by the formulations.  The rest is
-// pqp_dispatch_kernel's.
-__global__ void __launch_bounds__(kDispatchThreads)
-pqp_dispatch_forms_kernel(const __grid_constant__ DispatchArgs a, const __grid_constant__ pqp::FormTables t) {
-    extern __shared__ int32_t hist_s[];
-    __shared__ int32_t warp_sum[kDispatchThreads / 32];
-    int32_t *hist = a.hist ? a.hist : hist_s;
-    const int nsv = a.n_sets * a.nv, nb = nsv * a.ncols, tid = threadIdx.x;
-    for (int i = tid; i < nb; i += kDispatchThreads) hist[i] = 0;
-    if (tid == 0) a.n_view[a.batch] = 0;
-    __syncthreads();
-    for (int b = tid; b < a.batch; b += kDispatchThreads) {
-        const int n = a.n_points[b], off = a.offsets[b];
-        a.n_view[b] = n;
-        const int s = a.set ? a.set[b] : 0;
-        const int f = a.form_of[b];
-        const int keep = pqp::form_in_mask(f, a.form_mask) ? pqp::keep_control_steps(f, a.ref + off, n) : 0;
-        const int key = pqp::dispatch_key_forms(t, a.form_mask, f, s, a.n_sets, n, keep, a.min_keep, a.max_keep, a.nv,
-                                                a.ncols);
-        if (key >= 0) atomicAdd(&hist[key], 1);
-        else dispatch_reject(a, b, n, off);
-        a.key[b] = key;
-    }
-    __syncthreads();
-    dispatch_scatter(a, hist, nsv, a.ncols, warp_sum);
-}
-
 namespace {
 size_t dispatch_smem(int nv, int ncols) { return ((size_t)nv * ncols + nv) * sizeof(int32_t); }
+
+int max_ncols(const pqp_handle *h) { return std::max({h->cls_ncols[0], h->cls_ncols[1], h->cls_ncols[2]}); }
 
 // Which classes of `form` the stated bounds reach, the shortest path each of them can get and the shared memory it
 // needs: every (n, keep) inside the bounds, as class_for maps it.  Adds to `d` (min_n starts at INT32_MAX).
@@ -531,71 +506,79 @@ void reach_classes(const pqp_handle *h, pqp_handle::DispatchLaunches &d, int for
         }
 }
 
-// The classes one formulation's bounds reach, cached for the last bounds.
-void dispatch_launches(pqp_handle *h, int form, int max_n, int min_keep, int max_keep) {
-    pqp_handle::DispatchLaunches &d = h->disp;
-    if (d.valid && d.form == form && d.max_n == max_n && d.min_keep == min_keep && d.max_keep == max_keep) return;
-    d = pqp_handle::DispatchLaunches();
-    for (int v = 0; v < kNumVariants; ++v) d.min_n[v] = INT32_MAX;
-    reach_classes(h, d, form, max_n, min_keep, max_keep);
-    d.form = form; d.max_n = max_n; d.min_keep = min_keep; d.max_keep = max_keep;
-    d.valid = true;
-}
-
-// The same over the formulations of `form_mask`, formulation f bounded by max_n[f]; cached for the last (mask, bounds)
-// in a cache of its own, so that the single-formulation entries keep theirs.  Classes belong to one formulation each,
-// so every class gets exactly what dispatch_launches gives it for its formulation alone.
-void dispatch_launches_forms(pqp_handle *h, int form_mask, const int max_n[3], int min_keep, int max_keep) {
-    pqp_handle::DispatchLaunches &d = h->disp_forms;
-    if (d.valid && d.form == form_mask && std::equal(max_n, max_n + 3, d.max_n_form) && d.min_keep == min_keep &&
-        d.max_keep == max_keep)
-        return;
+// The classes the bounds reach over the formulations of `form_mask`, formulation f bounded by max_n[f].  Classes belong
+// to one formulation each, so every class gets exactly what its formulation's bounds give it alone.  Cached per (mask,
+// bounds) in PQP_DISPATCH_SLOTS slots, so that a caller alternating between masks or bounds keeps each of them.
+const pqp_handle::DispatchLaunches &dispatch_launches(pqp_handle *h, int form_mask, const int max_n[3], int min_keep,
+                                                      int max_keep) {
+    for (const pqp_handle::DispatchLaunches &d : h->disp)
+        if (d.valid && d.form_mask == form_mask && std::equal(max_n, max_n + 3, d.max_n) && d.min_keep == min_keep &&
+            d.max_keep == max_keep)
+            return d;
+    pqp_handle::DispatchLaunches &d = h->disp[h->disp_next];
+    h->disp_next = (h->disp_next + 1) % PQP_DISPATCH_SLOTS;
     d = pqp_handle::DispatchLaunches();
     for (int v = 0; v < kNumVariants; ++v) d.min_n[v] = INT32_MAX;
     for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC})
         if (pqp::form_in_mask(f, form_mask)) reach_classes(h, d, f, max_n[f], min_keep, max_keep);
-    d.form = form_mask; std::copy(max_n, max_n + 3, d.max_n_form); d.min_keep = min_keep; d.max_keep = max_keep;
+    d.form_mask = form_mask; std::copy(max_n, max_n + 3, d.max_n); d.min_keep = min_keep; d.max_keep = max_keep;
     d.valid = true;
+    return d;
+}
+
+// Room in the sort scratch for n_sets parameter sets (pqp_handle::d_disp_order / d_disp_hist).
+int dispatch_scratch(pqp_handle *h, int n_sets) {
+    if (n_sets <= h->disp_cap) return PQP_OK;
+    int cap = 1;
+    while (cap < n_sets) cap *= 2;
+    int32_t *o = nullptr, *hs = nullptr;
+    PQP_CUDA(cudaMalloc(&o, (size_t)cap * kNumVariants * h->max_batch * sizeof(int32_t)));
+    if (cudaMalloc(&hs, (size_t)cap * kNumVariants * (max_ncols(h) + 1) * sizeof(int32_t)) != cudaSuccess) {
+        cudaFree(o);
+        set_err("pqp_launch_dispatch: cudaMalloc of the sort scratch failed");
+        return PQP_ERR_CUDA;
+    }
+    if (h->d_disp_order) { h->retired.push_back(h->d_disp_order); h->retired.push_back(h->d_disp_hist); }
+    h->d_disp_order = o; h->d_disp_hist = hs; h->disp_cap = cap;
+    return PQP_OK;
 }
 }  // namespace
 
-int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
-                        int max_keep, cudaStream_t st, int *launches, const int32_t *d_set, int n_param_sets) {
-    dispatch_launches(h, form, max_n, min_keep, max_keep);
-    int v0, v1;
-    form_range(form, &v0, &v1);
-    const int nv = v1 - v0, ncols = h->cls_ncols[form];
-    // with a set index: every set below n_param_sets (0: all of them), order segments and histogram in global scratch
+int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form_mask, const int32_t *d_form, int batch,
+                        int total, const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
+                        const int32_t *d_set, int n_param_sets) {
+    // Layout: the order segments and the histogram span the classes [v_lo, v_hi) of the mask's formulations, with the
+    // largest ncols among them as the stride.  For one formulation that is its own classes and table width.
+    int v_lo = kNumVariants, v_hi = 0, ncols = 0;
+    DispatchArgs a;
+    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
+        a.t.table[f] = h->d_cls_table + h->cls_off[f];
+        a.t.ncols[f] = h->cls_ncols[f];
+        a.t.max_n[f] = pqp::form_in_mask(f, form_mask) ? max_n[f] : 0;   // (the reach cache's key as well)
+        if (!pqp::form_in_mask(f, form_mask)) continue;
+        int v0, v1;
+        form_range(f, &v0, &v1);
+        v_lo = std::min(v_lo, v0);
+        v_hi = std::max(v_hi, v1);
+        ncols = std::max(ncols, h->cls_ncols[f]);
+    }
+    const int nv = v_hi - v_lo;
+    const pqp_handle::DispatchLaunches &d = dispatch_launches(h, form_mask, a.t.max_n, min_keep, max_keep);
+    // with a set index: every set below n_param_sets (0: all of them), the histogram in global scratch
     int n_sets = 1;
-    int32_t *order = h->d_disp_order, *hist = nullptr;
     if (d_set) {
         n_sets = (int)h->dsets.size();
         if (n_param_sets > 0) n_sets = std::min(n_sets, n_param_sets);
-        if (n_sets > h->set_cap) {
-            int cap = 1;
-            while (cap < n_sets) cap *= 2;
-            int ncols_max = 0;
-            for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) ncols_max = std::max(ncols_max, h->cls_ncols[f]);
-            int32_t *o = nullptr, *hs = nullptr;
-            PQP_CUDA(cudaMalloc(&o, (size_t)cap * kNumKp * h->max_batch * sizeof(int32_t)));
-            if (cudaMalloc(&hs, (size_t)cap * kNumKp * (ncols_max + 1) * sizeof(int32_t)) != cudaSuccess) {
-                cudaFree(o);
-                set_err("pqp_launch_dispatch: cudaMalloc of the parameter-set sort scratch failed");
-                return PQP_ERR_CUDA;
-            }
-            if (h->d_set_order) { h->retired.push_back(h->d_set_order); h->retired.push_back(h->d_set_hist); }
-            h->d_set_order = o; h->d_set_hist = hs; h->set_cap = cap;
-        }
-        order = h->d_set_order;
-        hist = h->d_set_hist;
     }
+    const int rs = dispatch_scratch(h, n_sets);
+    if (rs != PQP_OK) return rs;
+    int32_t *order = h->d_disp_order, *hist = d_set ? h->d_disp_hist : nullptr;
     const size_t n_order = (size_t)n_sets * nv * batch;
     pqp_fill_kernel<<<(unsigned)std::min<size_t>((n_order + 255) / 256, 1024), 256, 0, st>>>(order, n_order, batch);
     PQP_CUDA(cudaGetLastError());
-    DispatchArgs a;
-    a.table = h->d_cls_table + h->cls_off[form];
-    a.ncols = ncols; a.form = form; a.v0 = v0; a.nv = nv;
-    a.max_n = max_n; a.min_keep = min_keep; a.max_keep = max_keep; a.batch = batch;
+    a.form_of = d_form; a.form = pqp::mask_form(form_mask); a.form_mask = form_mask;
+    a.v0 = v_lo; a.nv = nv; a.ncols = ncols;
+    a.min_keep = min_keep; a.max_keep = max_keep; a.batch = batch;
     a.n_points = bv.n_points; a.offsets = bv.offsets; a.ref = bv.ref;
     a.out_states = bv.out_states; a.out_frenet = bv.out_frenet; a.status = h->d_disp_status; a.iters = h->d_disp_iters;
     a.n_view = h->d_disp_n; a.key = h->d_disp_key; a.order = order;
@@ -609,13 +592,12 @@ int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int b
     // stations each, `total` in all); the CTAs past the segment's last path find the sentinel path and return.
     std::vector<int> count((size_t)n_sets * kNumVariants, 0), start((size_t)n_sets * kNumVariants, 0);
     std::vector<size_t> smem((size_t)n_sets * kNumVariants, 0);
-    const pqp_handle::DispatchLaunches &d = h->disp;
     for (int s = 0; s < n_sets; ++s)
-        for (int v = v0; v < v1; ++v) {
+        for (int v = v_lo; v < v_hi; ++v) {
             if (!d.reach[v]) continue;
             const int g = s * kNumVariants + v;
             count[g] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
-            start[g] = (s * nv + v - v0) * batch;
+            start[g] = (s * nv + v - v_lo) * batch;
             smem[g] = d.smem[v];
         }
     const int rc = launch_class_set(h, dv, n_sets, count.data(), start.data(), smem.data(), order, st, launches);
@@ -626,74 +608,45 @@ int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int b
     return PQP_OK;
 }
 
-int pqp_launch_dispatch_forms(pqp_handle *h, const pqp::BatchView &bv, int form_mask, int batch, int total,
-                              const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
-                              const int32_t *d_form, const int32_t *d_set, int n_param_sets) {
-    dispatch_launches_forms(h, form_mask, max_n, min_keep, max_keep);
-    int ncols = 0;
-    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) ncols = std::max(ncols, h->cls_ncols[f]);
-    const int nv = kNumVariants;
-    int n_sets = 1;
-    if (d_set) {
-        n_sets = (int)h->dsets.size();
-        if (n_param_sets > 0) n_sets = std::min(n_sets, n_param_sets);
+// The formulation checks of the single-formulation device entries.
+static int device_form_ok(int formulation, const double *d_max_k, const double *d_max_kp) {
+    if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
+        set_err("KPC needs d_max_k and d_max_kp (pqp_update_limits_device)");
+        return PQP_ERR_ARG;
     }
-    // order segments over every class (and, with a set index, the histogram) in grow-only scratch of their own: the
-    // single-formulation entries keep their buffers and layout
-    if (n_sets > h->form_cap) {
-        int cap = 1;
-        while (cap < n_sets) cap *= 2;
-        int32_t *o = nullptr, *hs = nullptr;
-        PQP_CUDA(cudaMalloc(&o, (size_t)cap * nv * h->max_batch * sizeof(int32_t)));
-        if (cudaMalloc(&hs, (size_t)cap * nv * (ncols + 1) * sizeof(int32_t)) != cudaSuccess) {
-            cudaFree(o);
-            set_err("pqp_launch_dispatch_forms: cudaMalloc of the formulation sort scratch failed");
-            return PQP_ERR_CUDA;
-        }
-        if (h->d_form_order) { h->retired.push_back(h->d_form_order); h->retired.push_back(h->d_form_hist); }
-        h->d_form_order = o; h->d_form_hist = hs; h->form_cap = cap;
+    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
+        set_err("unknown formulation");
+        return PQP_ERR_ARG;
     }
-    int32_t *order = h->d_form_order, *hist = d_set ? h->d_form_hist : nullptr;
-    const size_t n_order = (size_t)n_sets * nv * batch;
-    pqp_fill_kernel<<<(unsigned)std::min<size_t>((n_order + 255) / 256, 1024), 256, 0, st>>>(order, n_order, batch);
-    PQP_CUDA(cudaGetLastError());
-    DispatchArgs a;
-    a.table = nullptr;
-    a.ncols = ncols; a.form = -1; a.v0 = 0; a.nv = nv;
-    a.max_n = 0; a.min_keep = min_keep; a.max_keep = max_keep; a.batch = batch;
-    a.n_points = bv.n_points; a.offsets = bv.offsets; a.ref = bv.ref;
-    a.out_states = bv.out_states; a.out_frenet = bv.out_frenet; a.status = h->d_disp_status; a.iters = h->d_disp_iters;
-    a.n_view = h->d_disp_n; a.key = h->d_disp_key; a.order = order;
-    a.set = d_set; a.n_sets = n_sets; a.hist = hist;
-    a.form_of = d_form; a.form_mask = form_mask;
-    pqp::FormTables t;
-    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
-        t.table[f] = h->d_cls_table + h->cls_off[f];
-        t.ncols[f] = h->cls_ncols[f];
-        t.max_n[f] = max_n[f];
+    return PQP_OK;
+}
+
+// The BatchView and stream of a device entry's arguments (`stream` NULL: the handle's), once the batch fits the handle.
+static int device_batch(pqp_handle *h, int batch, int total_points, const int32_t *d_n_points, const int32_t *d_offsets,
+                        const pqp_state *d_ref, const pqp_station_bounds *d_bounds, const double *d_x0,
+                        const double *d_end_heading, const double *d_max_k, const double *d_max_kp,
+                        pqp_state *d_out_states, double *d_out_frenet, int32_t *d_status, int32_t *d_iters, void *stream,
+                        pqp::BatchView *bv, cudaStream_t *st) {
+    if (batch > h->max_batch || total_points > h->max_total) {
+        set_err("batch / total_points exceed what the handle was created for (workspace size)");
+        return PQP_ERR_CAPACITY;
     }
-    pqp_dispatch_forms_kernel<<<1, kDispatchThreads, hist ? 0 : dispatch_smem(nv, ncols), st>>>(a, t);
-    PQP_CUDA(cudaGetLastError());
-    if (launches) *launches += 2;
-    pqp::BatchView dv = bv;
-    dv.n_points = h->d_disp_n; dv.status = h->d_disp_status; dv.iters = h->d_disp_iters;
-    // grid per reached (set, class) exactly as pqp_launch_dispatch sizes it for the class's formulation alone
-    std::vector<int> count((size_t)n_sets * nv, 0), start((size_t)n_sets * nv, 0);
-    std::vector<size_t> smem((size_t)n_sets * nv, 0);
-    const pqp_handle::DispatchLaunches &d = h->disp_forms;
-    for (int s = 0; s < n_sets; ++s)
-        for (int v = 0; v < nv; ++v) {
-            if (!d.reach[v]) continue;
-            const int g = s * nv + v;
-            count[g] = d.min_n[v] >= 1 ? (int)std::min<long long>(batch, (long long)total / d.min_n[v]) : batch;
-            start[g] = g * batch;
-            smem[g] = d.smem[v];
-        }
-    const int rc = launch_class_set(h, dv, n_sets, count.data(), start.data(), smem.data(), order, st, launches);
-    if (rc != PQP_OK) return rc;
-    PQP_CUDA(cudaMemcpyAsync(bv.status, h->d_disp_status, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-    if (bv.iters)
-        PQP_CUDA(cudaMemcpyAsync(bv.iters, h->d_disp_iters, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    PQP_CUDA(cudaSetDevice(h->device));
+    *st = stream ? (cudaStream_t)stream : h->stream;
+    bv->batch = batch; bv->n_points = d_n_points; bv->offsets = d_offsets; bv->ref = d_ref; bv->bounds = d_bounds;
+    bv->x0 = d_x0; bv->end_heading = d_end_heading; bv->out_states = d_out_states; bv->out_frenet = d_out_frenet;
+    bv->status = d_status; bv->iters = d_iters; bv->workspace = h->d_ws; bv->debug = nullptr;
+    bv->max_k = d_max_k; bv->max_kp = d_max_kp;
+    return PQP_OK;
+}
+
+// The stats of a device entry: kernel_ms from h->ev[0], recorded on `st` before its launches, to their end (waited for).
+static int device_stats(pqp_handle *h, cudaStream_t st, int launches, pqp_stats *stats) {
+    memset(stats, 0, sizeof(*stats));
+    PQP_CUDA(cudaEventRecord(h->ev[1], st));
+    PQP_CUDA(cudaEventSynchronize(h->ev[1]));
+    PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
+    stats->kernel_launches = launches;
     return PQP_OK;
 }
 
@@ -778,10 +731,8 @@ void pqp_destroy(pqp_handle *h) {
     cudaFree(h->d_ref); cudaFree(h->d_out); cudaFree(h->d_bounds);
     cudaFree(h->d_x0); cudaFree(h->d_end); cudaFree(h->d_frenet); cudaFree(h->d_ws);
     cudaFree(h->d_max_k); cudaFree(h->d_max_kp);
-    cudaFree(h->d_cls_table); cudaFree(h->d_disp_order); cudaFree(h->d_disp_key);
+    cudaFree(h->d_cls_table); cudaFree(h->d_disp_order); cudaFree(h->d_disp_hist); cudaFree(h->d_disp_key);
     cudaFree(h->d_disp_n); cudaFree(h->d_disp_status); cudaFree(h->d_disp_iters);
-    cudaFree(h->d_set_order); cudaFree(h->d_set_hist);
-    cudaFree(h->d_form_order); cudaFree(h->d_form_hist);
     for (void *p : h->retired) cudaFree(p);
     cudaFreeHost(h->h_off); cudaFreeHost(h->h_order);
     cudaFree(h->d_gen); cudaFreeHost(h->h_gen);
@@ -872,26 +823,19 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
     PQP_TRY(cudaMalloc(&h->d_ws, pqp::kp2_ws_doubles(T, B) * sizeof(double)));
     PQP_TRY(cudaMallocHost(&h->h_off, (B + 1) * sizeof(int32_t)));
     PQP_TRY(cudaMallocHost(&h->h_order, B * sizeof(int32_t)));
-    // class tables of the device dispatch, uploaded once; order segments for the formulation with the most classes
+    // class tables of the device dispatch, uploaded once; its sort scratch for one parameter set
     {
         std::vector<int8_t> all, tab;
-        size_t smem = 0;
-        int ncols_max = 0;
         for (int form : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
-            int v0, v1;
-            form_range(form, &v0, &v1);
             h->cls_ncols[form] = class_table(h, form, &tab);
             h->cls_off[form] = (int)all.size();
             all.insert(all.end(), tab.begin(), tab.end());
-            smem = std::max(smem, dispatch_smem(v1 - v0, h->cls_ncols[form]));
-            ncols_max = std::max(ncols_max, h->cls_ncols[form]);
         }
         PQP_TRY(cudaMalloc(&h->d_cls_table, all.size()));
         PQP_TRY(cudaMemcpy(h->d_cls_table, all.data(), all.size(), cudaMemcpyHostToDevice));
-        PQP_TRY(cudaFuncSetAttribute(pqp_dispatch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PQP_TRY(cudaFuncSetAttribute(pqp_dispatch_forms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)dispatch_smem(kNumVariants, ncols_max)));
-        PQP_TRY(cudaMalloc(&h->d_disp_order, (size_t)kNumKp * B * sizeof(int32_t)));
+        PQP_TRY(cudaFuncSetAttribute(pqp_dispatch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)dispatch_smem(kNumVariants, max_ncols(h))));
+        if (dispatch_scratch(h, 1) != PQP_OK) return fail(PQP_ERR_CUDA);
         PQP_TRY(cudaMalloc(&h->d_disp_key, B * sizeof(int32_t)));
         PQP_TRY(cudaMalloc(&h->d_disp_n, (B + 1) * sizeof(int32_t)));
         PQP_TRY(cudaMalloc(&h->d_disp_status, (B + 1) * sizeof(int32_t)));
@@ -1014,36 +958,21 @@ int pqp_solve_batch_device(pqp_handle *h, int formulation, int batch, int total_
                            const double *d_max_k, const double *d_max_kp, pqp_state *d_out_states,
                            double *d_out_frenet, int32_t *d_status, int32_t *d_iters, void *stream,
                            pqp_stats *stats) {
-    (void)total_points;
     if (!h || batch < 0 || !d_n_points || !d_offsets || !d_ref || !d_bounds || !d_x0 || !d_end_heading ||
         !d_out_states || !d_status) {
         set_err("pqp_solve_batch_device: bad argument");
         return PQP_ERR_ARG;
     }
-    if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
-        set_err("KPC needs d_max_k and d_max_kp (pqp_update_limits_device)");
-        return PQP_ERR_ARG;
-    }
-    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        set_err("unknown formulation");
-        return PQP_ERR_ARG;
-    }
+    int rc = device_form_ok(formulation, d_max_k, d_max_kp);
+    if (rc != PQP_OK) return rc;
     if (batch == 0) return PQP_OK;
-    PQP_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     pqp::BatchView bv;
-    bv.batch = batch; bv.n_points = d_n_points; bv.offsets = d_offsets; bv.ref = d_ref; bv.bounds = d_bounds;
-    bv.x0 = d_x0; bv.end_heading = d_end_heading; bv.out_states = d_out_states; bv.out_frenet = d_out_frenet;
-    bv.status = d_status; bv.iters = d_iters;
-    bv.max_k = d_max_k; bv.max_kp = d_max_kp;
+    cudaStream_t st;
+    rc = device_batch(h, batch, total_points, d_n_points, d_offsets, d_ref, d_bounds, d_x0, d_end_heading, d_max_k,
+                      d_max_kp, d_out_states, d_out_frenet, d_status, d_iters, stream, &bv, &st);
+    if (rc != PQP_OK) return rc;
     // The host does not see n_points / keep here: the kernel shape class and the shared memory are
     // chosen from the caller's bounds; a path that does not fit reports PQP_INVALID_PROBLEM.
-    bv.workspace = h->d_ws;
-    bv.debug = nullptr;
-    if (batch > h->max_batch || total_points > h->max_total) {
-        set_err("batch / total_points exceed what the handle was created for (workspace size)");
-        return PQP_ERR_CAPACITY;
-    }
     const int nmax = max_n_points >= 2 ? max_n_points : std::min(h->max_total, 400);
     const int k_hi = (max_keep >= 1) ? std::min(max_keep, 10) : 4;
     const int k_lo = (min_keep >= 1) ? std::min(min_keep, k_hi) : 1;
@@ -1063,16 +992,9 @@ int pqp_solve_batch_device(pqp_handle *h, int formulation, int batch, int total_
         PQP_CUDA(cudaGetLastError());
         order = h->d_order_auto;
     }
-    int rc = launch_variant(h, v, &h->dprm, bv, batch, order, smem, st);
+    rc = launch_variant(h, v, &h->dprm, bv, batch, order, smem, st);
     if (rc != PQP_OK) return rc;
-    if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        PQP_CUDA(cudaEventRecord(h->ev[1], st));
-        PQP_CUDA(cudaEventSynchronize(h->ev[1]));
-        PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
-        stats->kernel_launches = ordered ? 2 : 1;
-    }
-    return PQP_OK;
+    return stats ? device_stats(h, st, ordered ? 2 : 1, stats) : PQP_OK;
 }
 
 int pqp_solve_batch_device_classes(pqp_handle *h, int formulation, int batch, int total_points,
@@ -1087,38 +1009,19 @@ int pqp_solve_batch_device_classes(pqp_handle *h, int formulation, int batch, in
         set_err("pqp_solve_batch_device_classes: bad argument");
         return PQP_ERR_ARG;
     }
-    if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
-        set_err("KPC needs d_max_k and d_max_kp (pqp_update_limits_device)");
-        return PQP_ERR_ARG;
-    }
-    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        set_err("unknown formulation");
-        return PQP_ERR_ARG;
-    }
+    int rc = device_form_ok(formulation, d_max_k, d_max_kp);
+    if (rc != PQP_OK) return rc;
     if (batch == 0) return PQP_OK;
-    if (batch > h->max_batch || total_points > h->max_total) {
-        set_err("batch / total_points exceed what the handle was created for (workspace size)");
-        return PQP_ERR_CAPACITY;
-    }
-    PQP_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     pqp::BatchView bv;
-    bv.batch = batch; bv.n_points = d_n_points; bv.offsets = d_offsets; bv.ref = d_ref; bv.bounds = d_bounds;
-    bv.x0 = d_x0; bv.end_heading = d_end_heading; bv.out_states = d_out_states; bv.out_frenet = d_out_frenet;
-    bv.status = d_status; bv.iters = d_iters; bv.workspace = h->d_ws; bv.debug = nullptr;
-    bv.max_k = d_max_k; bv.max_kp = d_max_kp;
+    cudaStream_t st;
+    rc = device_batch(h, batch, total_points, d_n_points, d_offsets, d_ref, d_bounds, d_x0, d_end_heading, d_max_k,
+                      d_max_kp, d_out_states, d_out_frenet, d_status, d_iters, stream, &bv, &st);
+    if (rc != PQP_OK) return rc;
     if (stats) PQP_CUDA(cudaEventRecord(h->ev[0], st));
     int launches = 0;
-    int rc = pqp_launch_kp_classes(h, bv, batch, h_n_points, nullptr, nullptr, h_keep, st, &launches, formulation);
+    rc = pqp_launch_kp_classes(h, bv, batch, h_n_points, nullptr, nullptr, h_keep, st, &launches, formulation);
     if (rc != PQP_OK) return rc;
-    if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        PQP_CUDA(cudaEventRecord(h->ev[1], st));
-        PQP_CUDA(cudaEventSynchronize(h->ev[1]));
-        PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
-        stats->kernel_launches = launches;
-    }
-    return PQP_OK;
+    return stats ? device_stats(h, st, launches, stats) : PQP_OK;
 }
 
 int pqp_solve_batch_device_dispatch(pqp_handle *h, int formulation, int batch, int total_points,
@@ -1145,39 +1048,21 @@ int pqp_solve_batch_device_dispatch_sets(pqp_handle *h, int formulation, int bat
         set_err("pqp_solve_batch_device_dispatch(_sets): bad argument");
         return PQP_ERR_ARG;
     }
-    if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
-        set_err("KPC needs d_max_k and d_max_kp (pqp_update_limits_device)");
-        return PQP_ERR_ARG;
-    }
-    if (formulation != PQP_FORM_KP && formulation != PQP_FORM_KPC && formulation != PQP_FORM_K) {
-        set_err("unknown formulation");
-        return PQP_ERR_ARG;
-    }
+    int rc = device_form_ok(formulation, d_max_k, d_max_kp);
+    if (rc != PQP_OK) return rc;
     if (batch == 0) return PQP_OK;
-    if (batch > h->max_batch || total_points > h->max_total) {
-        set_err("batch / total_points exceed what the handle was created for (workspace size)");
-        return PQP_ERR_CAPACITY;
-    }
-    PQP_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     pqp::BatchView bv;
-    bv.batch = batch; bv.n_points = d_n_points; bv.offsets = d_offsets; bv.ref = d_ref; bv.bounds = d_bounds;
-    bv.x0 = d_x0; bv.end_heading = d_end_heading; bv.out_states = d_out_states; bv.out_frenet = d_out_frenet;
-    bv.status = d_status; bv.iters = d_iters; bv.workspace = h->d_ws; bv.debug = nullptr;
-    bv.max_k = d_max_k; bv.max_kp = d_max_kp;
+    cudaStream_t st;
+    rc = device_batch(h, batch, total_points, d_n_points, d_offsets, d_ref, d_bounds, d_x0, d_end_heading, d_max_k,
+                      d_max_kp, d_out_states, d_out_frenet, d_status, d_iters, stream, &bv, &st);
+    if (rc != PQP_OK) return rc;
     if (stats) PQP_CUDA(cudaEventRecord(h->ev[0], st));
     int launches = 0;
-    int rc = pqp_launch_dispatch(h, bv, formulation, batch, total_points, max_n_points, min_keep, max_keep, st, &launches,
-                                 d_param_index, n_param_sets);
+    const int max_n[3] = {max_n_points, max_n_points, max_n_points};
+    rc = pqp_launch_dispatch(h, bv, 1 << formulation, nullptr, batch, total_points, max_n, min_keep, max_keep, st,
+                             &launches, d_param_index, n_param_sets);
     if (rc != PQP_OK) return rc;
-    if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        PQP_CUDA(cudaEventRecord(h->ev[1], st));
-        PQP_CUDA(cudaEventSynchronize(h->ev[1]));
-        PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
-        stats->kernel_launches = launches;
-    }
-    return PQP_OK;
+    return stats ? device_stats(h, st, launches, stats) : PQP_OK;
 }
 
 int pqp_solve_batch_device_dispatch_forms(pqp_handle *h, int batch, int total_points, int max_n_points, int min_keep,
@@ -1199,31 +1084,18 @@ int pqp_solve_batch_device_dispatch_forms(pqp_handle *h, int batch, int total_po
         return PQP_ERR_ARG;
     }
     if (batch == 0) return PQP_OK;
-    if (batch > h->max_batch || total_points > h->max_total) {
-        set_err("batch / total_points exceed what the handle was created for (workspace size)");
-        return PQP_ERR_CAPACITY;
-    }
-    PQP_CUDA(cudaSetDevice(h->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     pqp::BatchView bv;
-    bv.batch = batch; bv.n_points = d_n_points; bv.offsets = d_offsets; bv.ref = d_ref; bv.bounds = d_bounds;
-    bv.x0 = d_x0; bv.end_heading = d_end_heading; bv.out_states = d_out_states; bv.out_frenet = d_out_frenet;
-    bv.status = d_status; bv.iters = d_iters; bv.workspace = h->d_ws; bv.debug = nullptr;
-    bv.max_k = d_max_k; bv.max_kp = d_max_kp;
+    cudaStream_t st;
+    int rc = device_batch(h, batch, total_points, d_n_points, d_offsets, d_ref, d_bounds, d_x0, d_end_heading, d_max_k,
+                          d_max_kp, d_out_states, d_out_frenet, d_status, d_iters, stream, &bv, &st);
+    if (rc != PQP_OK) return rc;
     if (stats) PQP_CUDA(cudaEventRecord(h->ev[0], st));
     int launches = 0;
     const int max_n[3] = {max_n_points, max_n_points, max_n_points};
-    int rc = pqp_launch_dispatch_forms(h, bv, mask, batch, total_points, max_n, min_keep, max_keep, st, &launches,
-                                       d_formulation, d_param_index, n_param_sets);
+    rc = pqp_launch_dispatch(h, bv, mask, d_formulation, batch, total_points, max_n, min_keep, max_keep, st, &launches,
+                             d_param_index, n_param_sets);
     if (rc != PQP_OK) return rc;
-    if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        PQP_CUDA(cudaEventRecord(h->ev[1], st));
-        PQP_CUDA(cudaEventSynchronize(h->ev[1]));
-        PQP_CUDA(cudaEventElapsedTime(&stats->kernel_ms, h->ev[0], h->ev[1]));
-        stats->kernel_launches = launches;
-    }
-    return PQP_OK;
+    return stats ? device_stats(h, st, launches, stats) : PQP_OK;
 }
 
 int pqp_class_table(int formulation, int smem_optin, int8_t *table, int capacity, int *ncols) {
@@ -1480,29 +1352,20 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
         set_err("pqp_solve_batch_sets: no parameter-set index on a multi-device handle");
         return PQP_ERR_UNSUPPORTED;
     }
-    // offsets; launch segment (set * kNumVariants + shape class) and shared-memory need per path; segment G = the paths
-    // whose set index is out of range (rejected, not launched)
+    // offsets and keep_control_steps per path; launch segment set * kNumVariants + shape class, segment G = the paths
+    // whose set index or formulation is out of range (rejected, not launched)
     const int n_sets = param_index ? (int)h->dsets.size() : 1;
     const int G = n_sets * kNumVariants;
     long long total = 0;
     h->h_off[0] = 0;
-    std::vector<int> cls((size_t)batch);
-    std::vector<size_t> need_b((size_t)batch);
+    std::vector<int32_t> keep((size_t)batch);
     for (int b = 0; b < batch; ++b) {
         const int n = n_points[b];
         if (n < 0) { set_err("negative n_points"); return PQP_ERR_ARG; }
         total += n;
         if (total > h->max_total) { set_err("station count exceeds the handle's max_total_points"); return PQP_ERR_CAPACITY; }
         h->h_off[b + 1] = (int32_t)total;
-        const int s = param_index ? param_index[b] : 0;
-        const int f = forms ? forms[b] : formulation;
-        if (s < 0 || s >= n_sets || (forms && !pqp::form_in_mask(f, 7))) { cls[b] = G; need_b[b] = 0; continue; }
-        const int keep = (n >= 2) ? pqp_keep_control_steps(f, ref + h->h_off[b], n) : 1;
-        int v;
-        size_t need;
-        class_for(h, n, keep, &v, &need, f);
-        cls[b] = s * kNumVariants + v;
-        need_b[b] = need;
+        keep[b] = (n >= 2) ? pqp_keep_control_steps(forms ? forms[b] : formulation, ref + h->h_off[b], n) : 1;
     }
     // The batch is cut into contiguous chunks of paths that are pipelined over two streams: the
     // upload of chunk k+1 and the download of chunk k-1 overlap the kernels of chunk k (whose CTAs
@@ -1518,40 +1381,21 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
         cb[k] = (k == n_chunks) ? batch : std::max(b, cb[k - 1]);
     }
     h->plan.valid = false;   // (this call rewrites the order array the class plan of the device entry points refers to)
-    std::vector<double> okey;
-    if (batch <= kAutoOrderMax && auto_order_enabled()) {
-        okey.resize((size_t)batch);
-        for (int b = 0; b < batch; ++b) {
-            const int n = n_points[b];
-            okey[b] = n >= 1 ? order_key(n, x0[3 * (size_t)b], bounds[h->h_off[b]].c0_lb, bounds[h->h_off[b]].c0_ub) : 0.0;
-        }
+    // per chunk: per-segment order (written into the pinned order array at the chunk's range), the rejected paths last;
+    // small batches by the input-derived key, as pqp_order_kernel does on the device
+    const bool keyed = batch <= kAutoOrderMax && auto_order_enabled();
+    std::vector<double> okey(keyed ? (size_t)batch : 0);
+    for (int b = 0; keyed && b < batch; ++b) {
+        const int n = n_points[b];
+        okey[b] = n >= 1 ? order_key(n, x0[3 * (size_t)b], bounds[h->h_off[b]].c0_lb, bounds[h->h_off[b]].c0_ub) : 0.0;
     }
-    // per chunk: per-segment longest-first order (written into the pinned order array at the chunk's range), the
-    // rejected paths last
+    auto before = [&](int a, int b) { return keyed ? okey[a] > okey[b] : n_points[a] > n_points[b]; };
     std::vector<int> count_cv((size_t)n_chunks * (G + 1)), start_cv((size_t)n_chunks * (G + 2));
     std::vector<size_t> smem_cv((size_t)n_chunks * (G + 1));
-    for (int k = 0; k < n_chunks; ++k) {
-        int *count_k = count_cv.data() + (size_t)k * (G + 1), *start_k = start_cv.data() + (size_t)k * (G + 2);
-        size_t *smem_k = smem_cv.data() + (size_t)k * (G + 1);
-        for (int g = 0; g <= G; ++g) { count_k[g] = 0; smem_k[g] = 0; }
-        for (int b = cb[k]; b < cb[k + 1]; ++b) {
-            count_k[cls[b]]++;
-            smem_k[cls[b]] = std::max(smem_k[cls[b]], need_b[b]);
-        }
-        start_k[0] = cb[k];
-        for (int g = 0; g <= G; ++g) start_k[g + 1] = start_k[g] + count_k[g];
-        std::vector<int> fill(start_k, start_k + G + 1);
-        for (int b = cb[k]; b < cb[k + 1]; ++b) h->h_order[fill[cls[b]]++] = b;
-        const bool hinted = h->order_hint.size() == (size_t)batch;
-        const int32_t *hint = h->order_hint.data();
-        const bool keyed = !hinted && auto_order_enabled() && batch <= kAutoOrderMax;   // as pqp_order_kernel does on the device
-        for (int g = 0; g < G; ++g)
-            std::stable_sort(h->h_order + start_k[g], h->h_order + start_k[g + 1], [&](int a, int b) {
-                if (hinted) return (long long)n_points[a] * hint[a] > (long long)n_points[b] * hint[b];
-                if (keyed) return okey[a] > okey[b];
-                return n_points[a] > n_points[b];
-            });
-    }
+    for (int k = 0; k < n_chunks; ++k)
+        plan_classes(h, batch, cb[k], cb[k + 1], n_sets, n_points, keep.data(), formulation, forms, param_index, before,
+                     count_cv.data() + (size_t)k * (G + 1), start_cv.data() + (size_t)k * (G + 2),
+                     smem_cv.data() + (size_t)k * (G + 1));
     PQP_CUDA(cudaSetDevice(h->device));
     const size_t B = (size_t)batch, T = (size_t)total;
     pqp::BatchView bv;
@@ -1623,40 +1467,9 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
         // out on the class lanes (forked after the chunk's upload, joined before its download), longest class first, so
         // that they overlap instead of each waiting for the tail of the one before.
         const int *count_k = count_cv.data() + (size_t)k * (G + 1), *start_k = start_cv.data() + (size_t)k * (G + 2);
-        const size_t *smem_k = smem_cv.data() + (size_t)k * (G + 1);
-        int n_cls = 0;
-        for (int g = 0; g <= G; ++g) n_cls += count_k[g] > 0;
-        if (n_cls > 1) PQP_CUDA_DRAIN(cudaEventRecord(h->ev_fork, st));
-        int lane = 0;
-        for (int v = kNumVariants - 1; v >= 0; --v)
-            for (int s = 0; s < n_sets; ++s) {
-                const int g = s * kNumVariants + v;
-                if (!count_k[g]) continue;
-                cudaStream_t cs = st;
-                if (n_cls > 1) {
-                    cs = h->cls_stream[lane % PQP_CLASS_LANES];
-                    PQP_CUDA_DRAIN(cudaStreamWaitEvent(cs, h->ev_fork, 0));
-                    ++lane;
-                }
-                int rc = launch_variant(h, v, &h->dsets[s], bv, count_k[g], h->d_order + start_k[g], smem_k[g], cs);
-                if (rc != PQP_OK) { drain(); return rc; }
-                ++launches;
-            }
-        if (count_k[G]) {
-            cudaStream_t cs = st;
-            if (n_cls > 1) {
-                cs = h->cls_stream[lane % PQP_CLASS_LANES];
-                PQP_CUDA_DRAIN(cudaStreamWaitEvent(cs, h->ev_fork, 0));
-                ++lane;
-            }
-            pqp_reject_kernel<<<count_k[G], 128, 0, cs>>>(bv, h->d_order + start_k[G]);
-            PQP_CUDA_DRAIN(cudaGetLastError());
-            ++launches;
-        }
-        for (int j = 0; j < std::min(lane, PQP_CLASS_LANES); ++j) {
-            PQP_CUDA_DRAIN(cudaEventRecord(h->ev_cls[j], h->cls_stream[j]));
-            PQP_CUDA_DRAIN(cudaStreamWaitEvent(st, h->ev_cls[j], 0));
-        }
+        const int rc = launch_class_set(h, bv, n_sets, count_k, start_k, smem_cv.data() + (size_t)k * (G + 1), h->d_order,
+                                        st, &launches, count_k[G], start_k[G]);
+        if (rc != PQP_OK) { drain(); return rc; }
         PQP_CUDA_DRAIN(cudaEventRecord(h->ev_chunk[1 + k], st));   // this chunk's kernels done
         PQP_CUDA_DRAIN(cudaMemcpyAsync(out_states + o0, h->d_out + o0, nT * sizeof(pqp_state), cudaMemcpyDeviceToHost, st));
         if (out_frenet)

@@ -50,7 +50,7 @@ PQP_HD int dispatch_class(const int8_t *table, int ncols, int formulation, int n
     return table[row * ncols + col];
 }
 
-// Sort key of the device dispatch for a path of n stations on class `cls` (0-based within the formulation's nv classes)
+// Sort key of the device dispatch for a path of n stations on class `cls` (0-based within the nv classes the call spans)
 // with parameter set `set`: histogram bucket (set * nv + cls) * ncols + the longest-first length bucket.  The order
 // segment of the path is key / ncols = set * nv + cls, and ascending keys inside it run from the longest path down.
 PQP_HD int dispatch_key(int set, int cls, int nv, int ncols, int n) {
@@ -58,8 +58,8 @@ PQP_HD int dispatch_key(int set, int cls, int nv, int ncols, int n) {
     return (set * nv + cls) * ncols + (ncols - 1 - col);
 }
 
-// The dispatch over per-path formulations (the _forms entries): the class table, its ncols and the length bound of
-// every formulation, indexed by PQP_FORM_*.  max_n[f] = 0: unknown, as for dispatch_class.
+// The class table, its ncols and the length bound of every formulation, indexed by PQP_FORM_*.  max_n[f] = 0: unknown,
+// as for dispatch_class.
 struct FormTables {
     const int8_t *table[3];
     int ncols[3];
@@ -71,17 +71,24 @@ PQP_HD bool form_in_mask(int form, int form_mask) {
     return form >= 0 && form <= 2 && ((form_mask >> form) & 1);
 }
 
-// Sort key of the per-path-formulation dispatch for a path of `form`, n stations, keep_control_steps `keep` and
-// parameter set `set`: histogram bucket (set * n_variants + v) * ncols + the longest-first length bucket, where v is the
-// class index (global over the formulations, 0 .. n_variants - 1) the formulation's own table gives, and ncols is a
-// stride shared by every formulation (>= each table's ncols).  The order segment of the path is key / ncols, its class
-// (key / ncols) % n_variants.  -1 (no key: PQP_INVALID_PROBLEM) when the formulation is unknown or outside form_mask,
-// the set lies outside [0, n_sets), or the path lies outside its formulation's bounds.
+// The formulation of a one-bit form_mask: the single formulation of a call without a per-path array ("KP" for any other
+// mask, whose paths name their own).
+PQP_HD int mask_form(int form_mask) {
+    return form_mask == 1 << PQP_FORM_K ? PQP_FORM_K : form_mask == 1 << PQP_FORM_KPC ? PQP_FORM_KPC : PQP_FORM_KP;
+}
+
+// Sort key of the device dispatch for a path of `form`, n stations, keep_control_steps `keep` and parameter set `set`:
+// histogram bucket (set * n_variants + v - v_lo) * ncols + the longest-first length bucket, where v is the class (an
+// index of the whole variant space) the formulation's own table gives, [v_lo, v_lo + n_variants) the classes the
+// order spans (v_lo = 0: from the first class), and ncols a stride shared by the formulations in form_mask (>= each of
+// their tables' ncols).  The order segment of the path is key / ncols, its class v_lo + (key / ncols) % n_variants.
+// -1 (no key: PQP_INVALID_PROBLEM) when the formulation is unknown or outside form_mask, the set lies outside
+// [0, n_sets), or the path lies outside its formulation's bounds.
 PQP_HD int dispatch_key_forms(const FormTables &t, int form_mask, int form, int set, int n_sets, int n, int keep,
-                              int min_keep, int max_keep, int n_variants, int ncols) {
+                              int min_keep, int max_keep, int n_variants, int ncols, int v_lo = 0) {
     if (!form_in_mask(form, form_mask) || set < 0 || set >= n_sets) return -1;
     const int v = dispatch_class(t.table[form], t.ncols[form], form, n, keep, t.max_n[form], min_keep, max_keep);
-    return v < 0 ? -1 : dispatch_key(set, v, n_variants, ncols, n);
+    return v < 0 ? -1 : dispatch_key(set, v - v_lo, n_variants, ncols, n);
 }
 
 }  // namespace pqp

@@ -1109,19 +1109,19 @@ int pqp_densify_batch(pqp_handle *h, int batch, const int32_t *n_points, const p
 // pqp_plan_batch_maps uploads host buffers into the handle's, runs the body and downloads; pqp_plan_batch_device_maps
 // runs the body on the caller's device arrays.  pqp_plan_batch and pqp_plan_batch_device are the same with no index.
 struct ChainIO {
-    int formulation, bounds_mode, output_mode, batch;
+    int bounds_mode, output_mode, batch;
     int max_n;                      // >= every n_points[b]: sizes the bounds grid
     size_t total;
     PathsView paths;
     const int32_t *map_index;       // [batch] map of every path (bounds and collision check), NULL: map 0
     SetIndex set;                   // parameter set of every path (device index, NULL: set 0) and the sets it may name
     const int32_t *h_set;           // host copy of set.index (host class plan), else NULL
-    // per-path formulation (the _forms entries; `formulation` is then unused): the host array (host class plan) or the
-    // device array (device dispatch), NULL both without; form_mask = the formulations a path may name (1 << PQP_FORM_*)
-    // and max_n_form[f] the longest path of formulation f the device dispatch takes
-    const int32_t *h_form = nullptr, *d_form = nullptr;
+    // formulations: form_mask = the ones a path may name (1 << PQP_FORM_*), max_n_form[f] the longest path of formulation
+    // f the device dispatch takes, and the per-path array of the _forms entries: on the host (host class plan) or on the
+    // device (device dispatch).  A single-formulation call has a one-bit mask and no array.
     int form_mask = 0;
     int max_n_form[3] = {};
+    const int32_t *h_form = nullptr, *d_form = nullptr;
     const double *x0, *end_heading;
     double spacing;
     int collision_check, max_out;
@@ -1149,8 +1149,7 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
     bv.batch = c.batch; bv.n_points = e->d_nvalid; bv.offsets = c.paths.offsets; bv.ref = c.paths.ref; bv.bounds = c.bounds;
     bv.x0 = c.x0; bv.end_heading = c.end_heading; bv.out_states = c.qp_states; bv.out_frenet = nullptr;
     bv.status = c.status; bv.iters = c.iters; bv.workspace = h->d_ws; bv.debug = nullptr;
-    const bool mixed = c.h_form || c.d_form;
-    if (mixed ? pqp::form_in_mask(PQP_FORM_KPC, c.form_mask) : c.formulation == PQP_FORM_KPC) {
+    if (pqp::form_in_mask(PQP_FORM_KPC, c.form_mask)) {
         // updateLimits (reference_path_impl.cpp:203-235) between updateBounds and the QP, as solveWithoutSmoothing
         // does (path_optimizer.cpp:100-105): limits from the v, a fields of the reference states.  With per-path
         // formulations every path gets them; only the "KPC" paths read them.
@@ -1170,14 +1169,11 @@ static int run_chain(pqp_handle *h, EnvState *e, const ChainIO &c, const pqp_sta
         std::vector<int32_t> nv((size_t)c.batch);
         PQP_CUDA(cudaMemcpyAsync(nv.data(), e->d_nvalid, (size_t)c.batch * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
         PQP_CUDA(cudaStreamSynchronize(st));
-        rc = pqp_launch_kp_classes(h, bv, c.batch, nv.data(), h->h_off, h_ref, nullptr, st, qp_launches, c.formulation,
-                                   c.h_set, c.h_form);
-    } else if (c.d_form) {
-        rc = pqp_launch_dispatch_forms(h, bv, c.form_mask, c.batch, (int)c.total, c.max_n_form, 0, 0, st, qp_launches,
-                                       c.d_form, c.set.index, c.set.n_sets);
+        rc = pqp_launch_kp_classes(h, bv, c.batch, nv.data(), h->h_off, h_ref, nullptr, st, qp_launches,
+                                   pqp::mask_form(c.form_mask), c.h_set, c.h_form);
     } else {
-        rc = pqp_launch_dispatch(h, bv, c.formulation, c.batch, (int)c.total, c.max_n, 0, 0, st, qp_launches, c.set.index,
-                                 c.set.n_sets);
+        rc = pqp_launch_dispatch(h, bv, c.form_mask, c.d_form, c.batch, (int)c.total, c.max_n_form, 0, 0, st, qp_launches,
+                                 c.set.index, c.set.n_sets);
     }
     if (rc != PQP_OK) return rc;
     if (timed) PQP_CUDA(cudaEventRecord(e->ev[3], st));
@@ -1245,11 +1241,12 @@ static int plan_batch_host(pqp_handle *h, int formulation, const int32_t *forms,
         if (rc != PQP_OK) return rc;
     }
     ChainIO c;
-    c.formulation = formulation; c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
+    c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
     c.max_n = max_n; c.total = T; c.paths = handle_paths(h, e); c.map_index = map_index ? e->d_mapidx : nullptr;
     c.set = param_index ? SetIndex{e->d_setidx, (int)h->sets.size()} : kSet0;
     c.h_set = param_index;
     c.h_form = forms;
+    c.form_mask = forms ? 0 : 1 << formulation;
     for (int b = 0; forms && b < batch; ++b)
         if (pqp::form_in_mask(forms[b], 7)) c.form_mask |= 1 << forms[b];
     c.x0 = h->d_x0; c.end_heading = h->d_end;
@@ -1374,9 +1371,9 @@ int pqp_plan_batch_device_maps(pqp_handle *h, int formulation, int bounds_mode, 
 
 }  // extern "C"
 
-// The body of pqp_plan_batch_device_sets (d_form NULL) and pqp_plan_batch_device_forms (d_form [batch] on the device,
-// form_mask nonzero); arguments checked by the callers.
-static int plan_batch_device(pqp_handle *h, int formulation, int form_mask, const int32_t *d_form, int bounds_mode,
+// The body of pqp_plan_batch_device_sets (a one-bit form_mask, d_form NULL) and pqp_plan_batch_device_forms (d_form
+// [batch] on the device, form_mask nonzero); arguments checked by the callers.
+static int plan_batch_device(pqp_handle *h, int form_mask, const int32_t *d_form, int bounds_mode,
                              int output_mode, int batch, int total_points, int max_n_points, int n_param_sets,
                              const int32_t *d_n_points, const int32_t *d_offsets, const pqp_state *d_ref,
                              const int32_t *d_map_index, const int32_t *d_param_index, const int32_t *d_knot_offsets,
@@ -1396,18 +1393,13 @@ static int plan_batch_device(pqp_handle *h, int formulation, int form_mask, cons
     PQP_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     ChainIO c;
-    c.formulation = formulation; c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
-    // (0: the longest path any class of the formulation takes; a longer one reports PQP_INVALID_PROBLEM)
-    if (d_form) {
-        // every formulation of the mask bounded as its single-formulation call bounds it; the bounds grid covers the
-        // longest of them
-        c.d_form = d_form; c.form_mask = form_mask; c.max_n = 0;
-        for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
-            c.max_n_form[f] = max_n_points > 0 ? max_n_points : h->cls_ncols[f] - 2;
-            if (pqp::form_in_mask(f, form_mask)) c.max_n = std::max(c.max_n, c.max_n_form[f]);
-        }
-    } else {
-        c.max_n = max_n_points > 0 ? max_n_points : h->cls_ncols[formulation] - 2;
+    c.bounds_mode = bounds_mode; c.output_mode = output_mode; c.batch = batch;
+    // every formulation bounded by max_n_points (0: the longest path any of its classes takes; a longer one reports
+    // PQP_INVALID_PROBLEM); the bounds grid covers the longest bound of the mask
+    c.form_mask = form_mask; c.d_form = d_form; c.max_n = 0;
+    for (int f : {PQP_FORM_KP, PQP_FORM_K, PQP_FORM_KPC}) {
+        c.max_n_form[f] = max_n_points > 0 ? max_n_points : h->cls_ncols[f] - 2;
+        if (pqp::form_in_mask(f, form_mask)) c.max_n = std::max(c.max_n, c.max_n_form[f]);
     }
     c.total = (size_t)total_points;
     c.paths = PathsView{d_n_points, d_offsets, d_ref, d_knot_offsets, d_knots, d_x_coef, d_y_coef};
@@ -1465,7 +1457,7 @@ int pqp_plan_batch_device_sets(pqp_handle *h, int formulation, int bounds_mode, 
         pqp_set_err("pqp_plan_batch_device(_maps, _sets): unknown formulation");
         return PQP_ERR_ARG;
     }
-    return plan_batch_device(h, formulation, 0, nullptr, bounds_mode, output_mode, batch, total_points, max_n_points,
+    return plan_batch_device(h, 1 << formulation, nullptr, bounds_mode, output_mode, batch, total_points, max_n_points,
                              n_param_sets, d_n_points, d_offsets, d_ref, d_map_index, d_param_index, d_knot_offsets,
                              d_knots, d_x_coef, d_y_coef, d_x0, d_end_heading, output_spacing, collision_check, max_out,
                              d_out_states, d_out_n, d_out_ok, d_status, d_iters, d_out_bounds, stream, stats);
@@ -1488,7 +1480,7 @@ int pqp_plan_batch_device_forms(pqp_handle *h, int bounds_mode, int output_mode,
         pqp_set_err("pqp_plan_batch_device_forms: bad argument");
         return PQP_ERR_ARG;
     }
-    return plan_batch_device(h, PQP_FORM_KP, form_mask ? form_mask : 7, d_formulation, bounds_mode, output_mode, batch,
+    return plan_batch_device(h, form_mask ? form_mask : 7, d_formulation, bounds_mode, output_mode, batch,
                              total_points, max_n_points, n_param_sets, d_n_points, d_offsets, d_ref, d_map_index,
                              d_param_index, d_knot_offsets, d_knots, d_x_coef, d_y_coef, d_x0, d_end_heading,
                              output_spacing, collision_check, max_out, d_out_states, d_out_n, d_out_ok, d_status,

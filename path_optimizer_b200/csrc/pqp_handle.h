@@ -13,6 +13,7 @@
 #define PQP_MAX_CHUNKS 4
 #define PQP_CLASS_LANES 4
 #define PQP_MAX_VARIANTS 24
+#define PQP_DISPATCH_SLOTS 4
 
 struct pqp_handle {
     int device = 0;
@@ -42,10 +43,10 @@ struct pqp_handle {
     size_t dc_smem = 0;
     // class plan of the last pqp_launch_kp_classes call (reused while the batch shape stays the same)
     // launch segment g = set * (classes) + class; the entries past the last segment name the paths whose set index is
-    // out of range (n_reject of them)
+    // out of range (count[last] of them)
     struct ClassPlan {
         bool valid = false;
-        int skip = 0, form = 0, n_sets = 1, n_reject = 0;
+        int skip = 0, form = 0, n_sets = 1;
         cudaStream_t stream = nullptr;
         std::vector<int32_t> n, keep, set;   // (set: empty without a set index)
         std::vector<int32_t> forms;          // formulation of every path (empty without a per-path formulation)
@@ -55,34 +56,32 @@ struct pqp_handle {
     // pqp_set_order_hint: expected ADMM iterations per path (e.g. the previous planning cycle's counts); launch order
     // inside a class becomes longest-expected-first
     std::vector<int32_t> order_hint;
-    // device dispatch (pqp_solve_batch_device_dispatch, pqp_plan_batch_device): the class table of every formulation
-    // (pqp_dispatch.h; rows x cls_ncols[form] entries at d_cls_table + cls_off[form]), per-class order segments
-    // (max classes of a formulation x max_batch), one sort key per path, and the station counts, status and iterations
-    // the dispatched launches see: max_batch + 1 entries, the last one a path of 0 stations for unused order entries
+    // device dispatch (pqp_launch_dispatch): the class table of every formulation (pqp_dispatch.h; rows x
+    // cls_ncols[form] entries at d_cls_table + cls_off[form]), one sort key per path, and the station counts, status and
+    // iterations the dispatched launches see: max_batch + 1 entries, the last one a path of 0 stations for unused order
+    // entries
     int8_t *d_cls_table = nullptr;
     int cls_ncols[3] = {}, cls_off[3] = {};
-    int32_t *d_disp_order = nullptr, *d_disp_key = nullptr;
+    int32_t *d_disp_key = nullptr;
     int32_t *d_disp_n = nullptr, *d_disp_status = nullptr, *d_disp_iters = nullptr;
-    // device dispatch over parameter sets: per-(set, class) order segments (set_cap x max classes x max_batch) and the
-    // (set, class, length) histogram in global memory (it outgrows shared memory), grow-only.  An outgrown pair stays
-    // allocated until pqp_destroy: a graph captured before the growth still reads it.
-    int32_t *d_set_order = nullptr, *d_set_hist = nullptr;
-    int set_cap = 0;
-    // device dispatch over per-path formulations (the _forms entries): per-(set, class) order segments over every
-    // formulation's classes (form_cap x all classes x max_batch) and, with a set index, the (set, class, length)
-    // histogram (form_cap x all classes x (largest ncols + 1)); grow-only, outgrown buffers retired as above
-    int32_t *d_form_order = nullptr, *d_form_hist = nullptr;
-    int form_cap = 0;
+    // the dispatch's sort scratch, for disp_cap parameter sets: per-(set, class) order segments (disp_cap x every class
+    // x max_batch) and the (set, class, length) histogram, in global memory with a set index (disp_cap x every class x
+    // (largest ncols + 1)).  pqp_create allocates it for one set; it grows on
+    // demand and an outgrown pair stays allocated until pqp_destroy: a graph captured before the growth still reads it.
+    int32_t *d_disp_order = nullptr, *d_disp_hist = nullptr;
+    int disp_cap = 0;
     std::vector<void *> retired;
-    // launches of the last bounds the dispatch was asked for (form, max_n, min_keep, max_keep as passed)
+    // launches the dispatch makes for (form_mask, max_n per formulation, min_keep, max_keep as passed), for the last
+    // PQP_DISPATCH_SLOTS such bounds
     struct DispatchLaunches {
         bool valid = false;
-        int form = 0, max_n = 0, min_keep = 0, max_keep = 0;
-        int max_n_form[3] = {};   // (disp_forms: the bound of every formulation)
+        int form_mask = 0, min_keep = 0, max_keep = 0;
+        int max_n[3] = {};
         bool reach[PQP_MAX_VARIANTS] = {};
         int min_n[PQP_MAX_VARIANTS] = {};
         size_t smem[PQP_MAX_VARIANTS] = {};
-    } disp, disp_forms;   // disp_forms: the _forms entries, `form` holding their formulation mask
+    } disp[PQP_DISPATCH_SLOTS];
+    int disp_next = 0;
     // device buffers for the host-pointer entry point
     int32_t *d_n = nullptr, *d_off = nullptr, *d_order = nullptr, *d_status = nullptr, *d_iters = nullptr;
     int32_t *d_order_auto = nullptr;   // launch order computed on the device (pqp_solve_batch_device, small batches)
@@ -115,25 +114,21 @@ int pqp_launch_kp_classes(pqp_handle *h, const pqp::BatchView &bv, int batch, co
                           const int32_t *set = nullptr, const int32_t *forms = nullptr);
 
 // Internal (pqp_capi.cu): the same launches when the station counts exist on the device only.  A dispatch kernel reads
-// them, derives keep_control_steps from the device-side reference states, looks every path up in the class table and
-// sorts the paths into per-class order segments (longest first); every class the bounds can reach is launched over its
-// segment.  A path outside the bounds (max_n, min_keep..max_keep; 0 = unknown) reports PQP_INVALID_PROBLEM.
-// `total` = offsets[batch] bounds the grid of each class.  No host synchronisation, no allocation.
-// `d_set` [batch] (device): parameter set of every path, NULL: set 0; with it every (set < n_sets, class) pair the bounds
-// reach is launched, n_sets = min(n_param_sets, the handle's count) (n_param_sets 0: the handle's count).  A path whose set
-// lies outside [0, n_sets) reports PQP_INVALID_PROBLEM.
-int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form, int batch, int total, int max_n, int min_keep,
-                        int max_keep, cudaStream_t st, int *launches, const int32_t *d_set = nullptr, int n_param_sets = 0);
-
-// Internal (pqp_capi.cu): pqp_launch_dispatch over per-path formulations.  `d_form` [batch] (device) names every path's
-// formulation; `form_mask` (1 << PQP_FORM_*, nonzero) the ones launched: every (set, class) pair of those formulations
-// the bounds reach.  max_n[f] bounds the paths of formulation f (0: unknown); min_keep / max_keep apply to "KP".  A path
-// whose formulation lies outside the mask, or whose set or length lies outside the bounds, reports
-// PQP_INVALID_PROBLEM.  bv.max_k / max_kp must be set when the mask holds "KPC".  No allocation after a call with the
-// same or a larger set count.
-int pqp_launch_dispatch_forms(pqp_handle *h, const pqp::BatchView &bv, int form_mask, int batch, int total,
-                              const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
-                              const int32_t *d_form, const int32_t *d_set, int n_param_sets);
+// them, derives keep_control_steps from the device-side reference states, looks every path up in the class table of its
+// formulation and sorts the paths into per-(set, class) order segments (longest first); every (set, class) pair the
+// bounds can reach is launched over its segment.  No host synchronisation, and no allocation after a call with the same
+// or a smaller set count.
+// `form_mask` (1 << PQP_FORM_*, nonzero): the formulations launched.  `d_form` [batch] (device) names every path's
+// formulation; NULL: every path is the one formulation of a one-bit mask.  max_n[f] bounds the paths of formulation f
+// (0: unknown); min_keep / max_keep (0: unknown) apply to "KP".  bv.max_k / max_kp must be set when the mask holds "KPC".
+// `total` = offsets[batch] bounds the grid of each class.
+// `d_set` [batch] (device): parameter set of every path, NULL: set 0; with it every set below n_sets = min(n_param_sets,
+// the handle's count) (n_param_sets 0: the handle's count) is launched.
+// A path whose formulation lies outside the mask, or whose set or length lies outside the bounds, reports
+// PQP_INVALID_PROBLEM.
+int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form_mask, const int32_t *d_form, int batch,
+                        int total, const int max_n[3], int min_keep, int max_keep, cudaStream_t st, int *launches,
+                        const int32_t *d_set = nullptr, int n_param_sets = 0);
 
 // thread-local error text returned by pqp_last_error()
 extern thread_local char pqp_g_err[512];

@@ -29,8 +29,8 @@ def lib():
         L.env_emu_finish_raw_sets.argtypes = [pp, C.c_int, vp, dm, C.c_int, vp, C.c_int, vp, vp, C.c_int, vp, vp]
         L.env_emu_densify_sets.argtypes = ([pp, C.c_int, vp, dm, C.c_int, vp, C.c_int, vp, vp, C.c_double, C.c_int,
                                             C.c_int, vp, vp, vp])
-        L.sets_dispatch_emu.argtypes = [vp] + [C.c_int] * 6 + [vp] * 4 + [C.c_int] * 3 + [vp, vp]
-        for f in (L.env_emu_update_bounds_sets, L.env_emu_finish_raw_sets, L.env_emu_densify_sets, L.sets_dispatch_emu):
+        L.dispatch_sort_emu.argtypes = [vp, vp, vp, C.c_int, vp] + [C.c_int] * 5 + [vp] * 4 + [C.c_int] * 2 + [vp, vp]
+        for f in (L.env_emu_update_bounds_sets, L.env_emu_finish_raw_sets, L.env_emu_densify_sets, L.dispatch_sort_emu):
             f.restype = None
         _lib = L
     return _lib
@@ -99,7 +99,7 @@ def densify_sets(sets, set_index, maps, map_index, n_points, paths, output_spaci
 
 
 def sort(table, ncols, formulation, v0, nv, n_sets, batch, set_index, max_n=0, min_keep=0, max_keep=0):
-    """(order [n_sets, nv, B], key [B]) of the dispatch's (set, class) segment sort."""
+    """(order [n_sets, nv, B], key [B]) of the dispatch's (set, class) segment sort of one formulation."""
     n_points = np.ascontiguousarray(batch["n_points"], dtype=np.int32)
     B = len(n_points)
     offsets = np.ascontiguousarray(batch["offsets"], dtype=np.int32)
@@ -108,6 +108,8 @@ def sort(table, ncols, formulation, v0, nv, n_sets, batch, set_index, max_n=0, m
     table = np.ascontiguousarray(table, dtype=np.int8)
     order = np.zeros(n_sets * nv * B, dtype=np.int32)
     key = np.zeros(B, dtype=np.int32)
-    lib().sets_dispatch_emu(ptr(table), int(ncols), int(formulation), int(v0), int(nv), int(n_sets), B, ptr(n_points),
-                            ptr(offsets), ptr(ref), ptr(si), int(max_n), int(min_keep), int(max_keep), ptr(order), ptr(key))
+    lib().dispatch_sort_emu((C.c_void_p * 3)(*[table.ctypes.data] * 3), (C.c_int * 3)(*[ncols] * 3),
+                            (C.c_int * 3)(*[max_n] * 3), 1 << int(formulation), None, int(v0), int(nv), int(ncols),
+                            int(n_sets), B, ptr(n_points), ptr(offsets), ptr(ref), ptr(si), int(min_keep), int(max_keep),
+                            ptr(order), ptr(key))
     return order.reshape(n_sets, nv, B), key

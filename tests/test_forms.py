@@ -30,6 +30,8 @@ def harness(tmp_path_factory):
     L.forms_emu_key.restype = C.c_int
     L.forms_dispatch_emu.argtypes = [vp, vp, vp] + [C.c_int] * 5 + [vp] * 5 + [C.c_int] * 2 + [vp] * 2
     L.forms_dispatch_emu.restype = None
+    L.dispatch_sort_emu.argtypes = [vp, vp, vp, C.c_int, vp] + [C.c_int] * 5 + [vp] * 4 + [C.c_int] * 2 + [vp] * 2
+    L.dispatch_sort_emu.restype = None
     return L
 
 
@@ -56,6 +58,13 @@ class Tables:
     def key(self, H, form, n, keep, form_mask=ALL, set_=0, n_sets=1, min_keep=0, max_keep=0):
         return H.forms_emu_key(self.ptrs, self.ncols, self.max_n, form_mask, form, set_, n_sets, n, keep, min_keep,
                                max_keep, self.n_variants, self.stride)
+
+    def span(self, mask):
+        """(v_lo, nv, stride) of the device dispatch's order for `mask`: the classes its formulations select and the
+        widest of their tables."""
+        forms = [f for f in FORMS if (mask >> f) & 1]
+        vs = {_host_class(f, n, keep) for f in forms for keep in range(1, 12) for n in range(0, self.tabs[f][1])}
+        return min(vs), max(vs) + 1 - min(vs), max(self.tabs[f][1] for f in forms)
 
 
 def _host_class(form, n, keep):
@@ -115,40 +124,47 @@ def _mixed_batch(seed=5):
     return b, forms
 
 
-@pytest.mark.parametrize("n_sets,mask", [(1, ALL), (4, ALL), (3, (1 << shapes.KP) | (1 << shapes.KPC))])
+@pytest.mark.parametrize("n_sets,mask", [(1, ALL), (4, ALL), (3, (1 << shapes.KP) | (1 << shapes.KPC)),
+                                         (2, (1 << shapes.K) | (1 << shapes.KPC))])
 def test_segments_per_set_and_class_longest_first(harness, n_sets, mask):
+    """The sort in the order over every class, and in the span of the mask's classes that the device dispatch uses."""
     T = Tables()
     b, forms = _mixed_batch()
     B = len(forms)
     si = None if n_sets == 1 else (np.arange(B) % (n_sets + 1)).astype(np.int32)   # n_sets is out of range
-    order = np.zeros(n_sets * T.n_variants * B, dtype=np.int32)
-    key = np.zeros(B, dtype=np.int32)
     p = lambda a: None if a is None else np.ascontiguousarray(a).ctypes.data_as(C.c_void_p)  # noqa: E731
     ref = np.ascontiguousarray(b["ref"], dtype=STATE_DTYPE)
     n_points = np.ascontiguousarray(b["n_points"], dtype=np.int32)
     offsets = np.ascontiguousarray(b["offsets"], dtype=np.int32)
+    zeros = lambda nv: (np.zeros(n_sets * nv * B, dtype=np.int32), np.zeros(B, dtype=np.int32))  # noqa: E731
+    full = zeros(T.n_variants) + (0, T.n_variants, T.stride)
     harness.forms_dispatch_emu(T.ptrs, T.ncols, T.max_n, mask, T.n_variants, T.stride, n_sets, B, p(n_points), p(offsets),
-                               p(ref), p(si), p(forms), 0, 0, p(order), p(key))
-    order = order.reshape(n_sets, T.n_variants, B)
-    seen = {}
-    for s in range(n_sets):
-        for v in range(T.n_variants):
-            seg = order[s, v]
-            entries = seg[seg != B]
-            assert (seg[len(entries):] == B).all()
-            assert (np.diff(np.minimum(n_points[entries], T.stride - 1)) <= 0).all(), (s, v)
-            for i in entries:
-                assert int(i) not in seen
-                seen[int(i)] = (s, v)
+                               p(ref), p(si), p(forms), 0, 0, p(full[0]), p(full[1]))
+    v_lo, nv, stride = T.span(mask)
+    span = zeros(nv) + (v_lo, nv, stride)
+    harness.dispatch_sort_emu(T.ptrs, T.ncols, T.max_n, mask, p(forms), v_lo, nv, stride, n_sets, B, p(n_points),
+                              p(offsets), p(ref), p(si), 0, 0, p(span[0]), p(span[1]))
     L = _lib.load()
-    for i in range(B):
-        f, s = int(forms[i]), 0 if si is None else int(si[i])
-        if not (0 <= f <= 2 and (mask >> f) & 1 and 0 <= s < n_sets):
-            assert i not in seen and key[i] == -1, i
-            continue
-        r = ref[offsets[i]:offsets[i + 1]]
-        keep = L.pqp_keep_control_steps(f, r.ctypes.data_as(C.c_void_p), int(n_points[i]))
-        assert seen.get(i) == (s, _host_class(f, int(n_points[i]), keep)), i
+    for order, key, v_lo, nv, stride in (full, span):
+        order = order.reshape(n_sets, nv, B)
+        seen = {}
+        for s in range(n_sets):
+            for v in range(nv):
+                seg = order[s, v]
+                entries = seg[seg != B]
+                assert (seg[len(entries):] == B).all()
+                assert (np.diff(np.minimum(n_points[entries], stride - 1)) <= 0).all(), (s, v)
+                for i in entries:
+                    assert int(i) not in seen
+                    seen[int(i)] = (s, v_lo + v)
+        for i in range(B):
+            f, s = int(forms[i]), 0 if si is None else int(si[i])
+            if not (0 <= f <= 2 and (mask >> f) & 1 and 0 <= s < n_sets):
+                assert i not in seen and key[i] == -1, i
+                continue
+            r = ref[offsets[i]:offsets[i + 1]]
+            keep = L.pqp_keep_control_steps(f, r.ctypes.data_as(C.c_void_p), int(n_points[i]))
+            assert seen.get(i) == (s, _host_class(f, int(n_points[i]), keep)), i
 
 
 # ---- the ABI -------------------------------------------------------------------------------------------------------
