@@ -104,10 +104,15 @@ enum pqp_formulation {
 };
 
 /* Per-problem status: the OSQP status_val the reference would have seen.  The reference's
- * bool is (status == PQP_SOLVED): osqp-eigen's solve() returns false for anything else. */
+ * bool is (status == PQP_SOLVED): osqp-eigen's solve() returns false for anything else.
+ * At max_iter, when the last check has not stopped the run, OSQP 0.6 checks once more with eps_abs, eps_rel and
+ * eps_prim_inf x 10: PQP_SOLVED_INACCURATE when the residuals pass, PQP_PRIMAL_INFEASIBLE_INACCURATE when the
+ * infeasibility certificate holds, else PQP_MAX_ITER_REACHED.  PQP_SOLVED_INACCURATE and PQP_MAX_ITER_REACHED carry
+ * the last iterate; PQP_PRIMAL_INFEASIBLE and PQP_PRIMAL_INFEASIBLE_INACCURATE carry NaN. */
 enum pqp_status {
     PQP_SOLVED                 = 1,
     PQP_SOLVED_INACCURATE      = 2,
+    PQP_PRIMAL_INFEASIBLE_INACCURATE = 3,
     PQP_MAX_ITER_REACHED       = -2,
     PQP_PRIMAL_INFEASIBLE      = -3,
     PQP_DUAL_INFEASIBLE        = -4,
@@ -188,6 +193,15 @@ int pqp_problem_size(int formulation, int n_points, int keep, int *n_var, int *n
  * (solver.hpp:52) that every reference solve constructs from scratch. */
 int pqp_create(pqp_handle **out, const pqp_params *params, int device,
                int max_batch, int max_total_points);
+
+/* OSQP settings.  pqp_create, pqp_set_params and pqp_set_param_sets refuse, with PQP_ERR_ARG, the settings that OSQP
+ * 0.6's osqp_setup refuses (validate_settings), so that a solve never runs where the reference's solve() would have
+ * failed at setup:
+ *   rho > 0, sigma > 0, 0 < alpha < 2, max_iter > 0,
+ *   eps_abs >= 0 and eps_rel >= 0, not both 0, eps_prim_inf > 0, eps_dual_inf > 0,
+ *   scaling >= 0, check_termination >= 0,
+ *   adaptive_rho 0 or 1, adaptive_rho_interval >= 0, adaptive_rho_tolerance >= 1.
+ * A NaN in any of these fields is refused. */
 
 void pqp_destroy(pqp_handle *h);
 

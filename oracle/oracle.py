@@ -20,7 +20,7 @@ _LIB_PATH = os.path.join(_HERE, "_build", "libpqp_oracle.so")
 class OqpInfo(C.Structure):
     _fields_ = [("status", C.c_int), ("iters", C.c_int), ("rho_updates", C.c_int),
                 ("rho_final", C.c_double), ("pri_res", C.c_double), ("dua_res", C.c_double),
-                ("obj_val", C.c_double), ("kkt_n", C.c_int), ("kkt_lnz", C.c_int)]
+                ("obj_val", C.c_double), ("kkt_n", C.c_int), ("kkt_lnz", C.c_int), ("margin", C.c_double)]
 
 
 class OqpProblem(C.Structure):

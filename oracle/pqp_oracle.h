@@ -49,6 +49,9 @@ typedef struct oqp_info {
     double pri_res, dua_res;
     double obj_val;
     int kkt_n, kkt_lnz;    /* size of the KKT system and nnz(L) */
+    double margin;         /* the deciding check(s) -- the one that stopped the run, or the last one and the 10x
+                              re-check at max_iter: smallest relative gap |a - b| / max(|a|, |b|) of a residual or
+                              certificate value a from its threshold b (0 when nothing was checked) */
 } oqp_info;
 
 /* Flag defaults, restated from src/config/planning_flags.cpp:18-119 + updateConfig() :8-14,

@@ -423,7 +423,14 @@ typedef struct {
     double *x, *z, *y, *x_prev, *z_prev, *xz_tilde, *rhs;
     double *Ax, *Px, *Aty, *delta_x, *delta_y, *Adelta_x, *Atdelta_y, *Pdelta_x;
     double *D_temp, *D_temp_A, *E_temp;
+    double margin;         /* smallest relative gap of a value from its threshold in the checks since the last reset */
 } work;
+
+/* relative distance of a compared value from its threshold: a verdict closer than rounding is a coin flip */
+static void note_gap(work *w, double a, double b) {
+    const double d = c_max(c_absval(a), c_absval(b));
+    w->margin = c_min(w->margin, d > 0 ? c_absval(a - b) / d : 0.0);
+}
 
 static void scale_data(work *w, int sweeps) {
     const int n = w->n, m = w->m;
@@ -563,13 +570,17 @@ static int is_primal_infeasible(work *w, double eps_prim_inf) {
         }
     }
     double norm_delta_y = vec_scaled_norm_inf(w->E, w->delta_y, m);
+    note_gap(w, norm_delta_y, eps_prim_inf);
     if (norm_delta_y > eps_prim_inf) {
         double ineq_lhs = 0;
         for (int i = 0; i < m; ++i)
             ineq_lhs += w->u[i] * c_max(w->delta_y[i], 0) + w->l[i] * c_min(w->delta_y[i], 0);
+        note_gap(w, ineq_lhs, -eps_prim_inf * norm_delta_y);
         if (ineq_lhs < -eps_prim_inf * norm_delta_y) {
             mat_tpose_vec(w->A, w->delta_y, w->Atdelta_y);
-            return vec_scaled_norm_inf(w->Dinv, w->Atdelta_y, n) < eps_prim_inf * norm_delta_y;
+            const double cert = vec_scaled_norm_inf(w->Dinv, w->Atdelta_y, n);
+            note_gap(w, cert, eps_prim_inf * norm_delta_y);
+            return cert < eps_prim_inf * norm_delta_y;
         }
     }
     return 0;
@@ -609,16 +620,30 @@ static int check_termination(work *w, const pqp_params *prm, double pri_res, dou
     if (w->m == 0) prim_res_check = 1;
     else {
         double eps_prim = compute_pri_tol(w, eps_abs, eps_rel);
+        note_gap(w, pri_res, eps_prim);
         if (pri_res < eps_prim) prim_res_check = 1;
         else prim_inf_check = is_primal_infeasible(w, eps_prim_inf);
     }
     double eps_dual = compute_dua_tol(w, eps_abs, eps_rel);
+    note_gap(w, dua_res, eps_dual);
     if (dua_res < eps_dual) dual_res_check = 1;
     else dual_inf_check = is_dual_infeasible(w, eps_dual_inf);
     if (prim_res_check && dual_res_check) { *status = approximate ? PQP_SOLVED_INACCURATE : PQP_SOLVED; return 1; }
-    if (prim_inf_check) { *status = PQP_PRIMAL_INFEASIBLE; return 1; }
+    if (prim_inf_check) { *status = approximate ? PQP_PRIMAL_INFEASIBLE_INACCURATE : PQP_PRIMAL_INFEASIBLE; return 1; }
     if (dual_inf_check) { *status = PQP_DUAL_INFEASIBLE; return 1; }
     return 0;
+}
+
+/* OSQP 0.6 validate_settings (auxil.c), on the settings pqp_params carries; written so that a NaN fails */
+static int settings_valid(const pqp_params *p) {
+    if (!(p->rho > 0) || !(p->sigma > 0) || !(p->alpha > 0) || !(p->alpha < 2)) return 0;
+    if (!(p->max_iter > 0)) return 0;
+    if (!(p->eps_abs >= 0) || !(p->eps_rel >= 0) || (p->eps_abs == 0 && p->eps_rel == 0)) return 0;
+    if (!(p->eps_prim_inf > 0) || !(p->eps_dual_inf > 0)) return 0;
+    if (p->scaling < 0 || p->check_termination < 0) return 0;
+    if (p->adaptive_rho != 0 && p->adaptive_rho != 1) return 0;
+    if (p->adaptive_rho_interval < 0 || !(p->adaptive_rho_tolerance >= 1)) return 0;
+    return 1;
 }
 
 static double compute_rho_estimate(const work *w) {
@@ -640,14 +665,15 @@ int oracle_osqp_solve(const pqp_params *prm, const oqp_problem *qp, double *x_ou
     if (!info) info = &local;
     memset(info, 0, sizeof(*info));
     info->status = PQP_UNSOLVED;
-    /* osqp_setup -> validate_data: lower bound greater than upper bound is refused */
-    for (int i = 0; i < m; ++i)
-        if (!(qp->l[i] <= qp->u[i])) {
-            info->status = PQP_INVALID_PROBLEM;
-            for (int k = 0; k < n; ++k) x_out[k] = NAN;
-            if (y_out) for (int k = 0; k < m; ++k) y_out[k] = NAN;
-            return info->status;
-        }
+    /* osqp_setup refuses settings that fail validate_settings and bounds with l > u (validate_data) */
+    int refused = !settings_valid(prm);
+    for (int i = 0; i < m && !refused; ++i) refused = !(qp->l[i] <= qp->u[i]);
+    if (refused) {
+        info->status = PQP_INVALID_PROBLEM;
+        for (int k = 0; k < n; ++k) x_out[k] = NAN;
+        if (y_out) for (int k = 0; k < m; ++k) y_out[k] = NAN;
+        return info->status;
+    }
     work W;
     work *w = &W;
     memset(w, 0, sizeof(W));
@@ -728,6 +754,7 @@ int oracle_osqp_solve(const pqp_params *prm, const oqp_problem *qp, double *x_ou
                     if (row < trace_cap)
                         for (int i = 0; i < n; ++i) trace[(size_t)row * n + i] = w->D[i] * w->x[i];
                 }
+                w->margin = INFINITY;
                 if (check_termination(w, prm, pri_res, dua_res, 0, &status)) break;
             }
             if (prm->adaptive_rho && prm->adaptive_rho_interval &&
@@ -760,6 +787,7 @@ int oracle_osqp_solve(const pqp_params *prm, const oqp_problem *qp, double *x_ou
             if (!can_check) {
                 pri_res = compute_pri_res(w, w->x, w->z);
                 dua_res = compute_dua_res(w, w->x, w->y);
+                w->margin = INFINITY;
                 check_termination(w, prm, pri_res, dua_res, 0, &status);
             }
             if (status == PQP_UNSOLVED) {
@@ -772,6 +800,7 @@ int oracle_osqp_solve(const pqp_params *prm, const oqp_problem *qp, double *x_ou
     info->rho_final = w->rho;
     info->pri_res = pri_res;
     info->dua_res = dua_res;
+    info->margin = w->margin;
     /* store_solution: unscale; NaN when the status carries no solution */
     if (status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED) {
         for (int i = 0; i < n; ++i) x_out[i] = w->D[i] * w->x[i];

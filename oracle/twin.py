@@ -273,17 +273,27 @@ def _limit(v):
     return np.where(v > MAX_SCALING, MAX_SCALING, v)
 
 
+def _rel_gap(a, b):
+    """Relative distance of a compared value from its threshold (0 when the comparison is a coin flip)."""
+    d = max(abs(a), abs(b))
+    return abs(a - b) / d if d > 0 else 0.0
+
+
 def osqp_twin(prm, P, q, A, l, u, eps=None, max_iter=None, trace_every=0):
-    """OSQP 0.6.x recurrence on dense/sparse (P full symmetric, A).  Returns dict(x, y, iters,
-    status, rho_updates, trace)."""
+    """OSQP 0.6.x recurrence on dense/sparse (P full symmetric, A), through the end of osqp_solve: the checks inside
+    the loop, the exact check after it when the last iteration was not a check iteration, and the re-check with
+    eps_abs, eps_rel and eps_prim_inf x 10 when nothing has stopped the run.  Returns dict(x, y, iters, status,
+    rho_updates, rho, trace, decision): x and y are NaN when the status carries no solution (store_solution), and
+    `decision` holds the residuals and tolerances of the deciding check(s) with `margin`, the smallest relative gap
+    between a compared value and its threshold there."""
     P = sp.csc_matrix(P); A = sp.csc_matrix(A)
     n, m = P.shape[0], A.shape[0]
     q = np.array(q, dtype=float); l = np.array(l, dtype=float); u = np.array(u, dtype=float)
-    if np.any(l > u):
-        return dict(x=np.full(n, np.nan), y=np.full(m, np.nan), iters=0, status=-100, rho_updates=0)
     eps_abs = prm.eps_abs if eps is None else eps
     eps_rel = prm.eps_rel if eps is None else eps
     max_iter = prm.max_iter if max_iter is None else max_iter
+    if np.any(l > u) or max_iter < 1:
+        return dict(x=np.full(n, np.nan), y=np.full(m, np.nan), iters=0, status=-100, rho_updates=0)
     D = np.ones(n); E = np.ones(m); c = 1.0
     for _ in range(prm.scaling):
         absP, absA = abs(P), abs(A)
@@ -320,11 +330,53 @@ def osqp_twin(prm, P, q, A, l, u, eps=None, max_iter=None, trace_every=0):
 
     rho_vec = rho_vector(rho)
     lu = factor(rho_vec)
-    x = np.zeros(n); z = np.zeros(m); y = np.zeros(m)
+    x = np.zeros(n); z = np.zeros(m); y = np.zeros(m); dy = np.zeros(m)
     Dinv, Einv, cinv = 1.0 / D, 1.0 / E, 1.0 / c
-    status, rho_updates, it = -10, 0, 0
-    trace = []
     ninf = lambda v: np.abs(v).max() if len(v) else 0.0  # noqa: E731
+    uinf, linf = u > INFTY * MIN_SCALING, l < -INFTY * MIN_SCALING
+
+    def residuals():
+        Ax = A @ x; Px = P @ x; Aty = A.T @ y
+        return dict(Ax=Ax, Px=Px, Aty=Aty, rp=Ax - z, rd=q + Px + Aty,
+                    pri_res=ninf(Einv * (Ax - z)), dua_res=cinv * ninf(Dinv * (q + Px + Aty)))
+
+    def check(r, approximate, gaps):
+        """check_termination(work, approximate): a status, or None to go on.  q = 0 for this path, so the dual
+        infeasibility certificate is dead.  Appends the relative gap of every comparison it makes to `gaps`."""
+        k = 10.0 if approximate else 1.0
+        ea, er, ep = k * eps_abs, k * eps_rel, k * prm.eps_prim_inf
+        if r["pri_res"] > INFTY or r["dua_res"] > INFTY:
+            return -7
+        eps_p = ea + er * max(ninf(Einv * z), ninf(Einv * r["Ax"]))
+        eps_d = ea + er * cinv * max(ninf(Dinv * q), ninf(Dinv * r["Aty"]), ninf(Dinv * r["Px"]))
+        r.update(eps_pri=eps_p, eps_dua=eps_d)
+        prim_ok = r["pri_res"] < eps_p
+        dua_ok = r["dua_res"] < eps_d
+        gaps += [_rel_gap(r["pri_res"], eps_p), _rel_gap(r["dua_res"], eps_d)]
+        if prim_ok and dua_ok:
+            return 2 if approximate else 1
+        if not prim_ok:
+            # primal infeasibility certificate on delta y, projected onto the polar of the bounds' recession cone
+            d = dy.copy()
+            d[uinf & linf] = 0
+            d[uinf & ~linf] = np.minimum(d[uinf & ~linf], 0)
+            d[~uinf & linf] = np.maximum(d[~uinf & linf], 0)
+            nd = ninf(E * d)
+            gaps.append(_rel_gap(nd, ep))
+            if nd > ep:
+                lhs = np.sum(u * np.maximum(d, 0) + l * np.minimum(d, 0))
+                gaps.append(_rel_gap(lhs, -ep * nd))
+                if lhs < -ep * nd:
+                    cert = ninf(Dinv * (A.T @ d))
+                    gaps.append(_rel_gap(cert, ep * nd))
+                    if cert < ep * nd:
+                        return 3 if approximate else -3
+        return None
+
+    status, rho_updates, it = None, 0, 0
+    trace = []
+    r, gaps = None, []
+    can_check = False
     for it in range(1, max_iter + 1):
         xp, zp = x, z
         rhs = np.concatenate([prm.sigma * xp - q, zp - y / rho_vec])
@@ -336,46 +388,41 @@ def osqp_twin(prm, P, q, A, l, u, eps=None, max_iter=None, trace_every=0):
         z = np.minimum(np.maximum(zr + y / rho_vec, l), u)
         dy = rho_vec * (zr - z)
         y = y + dy
-        can_check = prm.check_termination and it % prm.check_termination == 0
+        can_check = bool(prm.check_termination) and it % prm.check_termination == 0
         can_adapt = prm.adaptive_rho and prm.adaptive_rho_interval and it % prm.adaptive_rho_interval == 0
         if can_check or can_adapt:
-            Ax = A @ x; Px = P @ x; Aty = A.T @ y
-            rp = Ax - z; rd = q + Px + Aty
-            pri_res = ninf(Einv * rp); dua_res = cinv * ninf(Dinv * rd)
+            r = residuals()
         if can_check:
             if trace_every and (it // prm.check_termination) % trace_every == 0:
                 trace.append(D * x)
-            eps_p = eps_abs + eps_rel * max(ninf(Einv * z), ninf(Einv * Ax))
-            eps_d = eps_abs + eps_rel * cinv * max(ninf(Dinv * q), ninf(Dinv * Aty), ninf(Dinv * Px))
-            if pri_res < eps_p and dua_res < eps_d:
-                status = 1
+            gaps = []
+            status = check(r, False, gaps)
+            if status is not None:
                 break
-            # primal infeasibility certificate (q = 0 for this path, so the dual one is dead)
-            if not pri_res < eps_p:
-                d = dy.copy()
-                uinf, linf = u > INFTY * MIN_SCALING, l < -INFTY * MIN_SCALING
-                d[uinf & linf] = 0
-                d[uinf & ~linf] = np.minimum(d[uinf & ~linf], 0)
-                d[~uinf & linf] = np.maximum(d[~uinf & linf], 0)
-                nd = ninf(E * d)
-                if nd > prm.eps_prim_inf:
-                    lhs = np.sum(u * np.maximum(d, 0) + l * np.minimum(d, 0))
-                    if lhs < -prm.eps_prim_inf * nd and ninf(Dinv * (A.T @ d)) < prm.eps_prim_inf * nd:
-                        status = -3
-                        break
         if can_adapt:
-            pn = ninf(rp) / (max(ninf(z), ninf(Ax)) + 1e-10)
-            dn = ninf(rd) / (max(ninf(q), ninf(Aty), ninf(Px)) + 1e-10)
+            pn = ninf(r["rp"]) / (max(ninf(z), ninf(r["Ax"])) + 1e-10)
+            dn = ninf(r["rd"]) / (max(ninf(q), ninf(r["Aty"]), ninf(r["Px"])) + 1e-10)
             rho_new = min(max(rho * np.sqrt(pn / (dn + 1e-10)), RHO_MIN), RHO_MAX)
             if rho_new > rho * prm.adaptive_rho_tolerance or rho_new < rho / prm.adaptive_rho_tolerance:
                 rho = rho_new
                 rho_vec = rho_vector(rho)
                 lu = factor(rho_vec)
                 rho_updates += 1
-    if status == -10:
-        status = -2
-    return dict(x=D * x, y=cinv * E * y, iters=it, status=status, rho_updates=rho_updates,
-                rho=rho, trace=np.array(trace))
+    exact = None
+    if status is None:
+        if not can_check:                   # the last iteration was not a check iteration: check it exactly now
+            r, gaps = residuals(), []
+            status = check(r, False, gaps)
+        if status is None:                  # max_iter reached: the 10x re-check
+            exact = dict(pri_res=r["pri_res"], dua_res=r["dua_res"], eps_pri=r["eps_pri"], eps_dua=r["eps_dua"])
+            status = check(r, True, gaps)
+            if status is None:
+                status = -2
+    decision = dict(pri_res=r["pri_res"], dua_res=r["dua_res"], eps_pri=r.get("eps_pri"), eps_dua=r.get("eps_dua"),
+                    exact=exact, margin=min(gaps) if gaps else np.inf)
+    has_sol = status in (1, 2, -2)
+    return dict(x=D * x if has_sol else np.full(n, np.nan), y=cinv * E * y if has_sol else np.full(m, np.nan),
+                iters=it, status=status, rho_updates=rho_updates, rho=rho, trace=np.array(trace), decision=decision)
 
 
 def kkt_certificate(P, q, A, l, u, x, y):

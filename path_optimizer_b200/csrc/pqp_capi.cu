@@ -608,6 +608,25 @@ int pqp_launch_dispatch(pqp_handle *h, const pqp::BatchView &bv, int form_mask, 
     return PQP_OK;
 }
 
+// OSQP 0.6's validate_settings on the settings pqp_params carries (pqp.h): false, with the rule in pqp_last_error(),
+// where osqp_setup would refuse them.  Every test is written so that a NaN fails it.
+static bool settings_ok(const pqp_params &p, const char *entry) {
+    const char *bad = !(p.rho > 0) ? "rho > 0"
+                      : !(p.sigma > 0) ? "sigma > 0"
+                      : !(p.alpha > 0 && p.alpha < 2) ? "0 < alpha < 2"
+                      : !(p.max_iter > 0) ? "max_iter > 0"
+                      : !(p.eps_abs >= 0 && p.eps_rel >= 0) ? "eps_abs >= 0 and eps_rel >= 0"
+                      : (p.eps_abs == 0 && p.eps_rel == 0) ? "eps_abs and eps_rel not both 0"
+                      : !(p.eps_prim_inf > 0 && p.eps_dual_inf > 0) ? "eps_prim_inf > 0 and eps_dual_inf > 0"
+                      : !(p.scaling >= 0 && p.check_termination >= 0) ? "scaling >= 0 and check_termination >= 0"
+                      : !(p.adaptive_rho == 0 || p.adaptive_rho == 1) ? "adaptive_rho 0 or 1"
+                      : !(p.adaptive_rho_interval >= 0) ? "adaptive_rho_interval >= 0"
+                      : !(p.adaptive_rho_tolerance >= 1) ? "adaptive_rho_tolerance >= 1"
+                      : nullptr;
+    if (bad) set_err("%s: OSQP refuses these settings (needs %s)", entry, bad);
+    return !bad;
+}
+
 // The formulation checks of the single-formulation device entries.
 static int device_form_ok(int formulation, const double *d_max_k, const double *d_max_kp) {
     if (formulation == PQP_FORM_KPC && (!d_max_k || !d_max_kp)) {
@@ -752,6 +771,8 @@ int pqp_set_param_sets(pqp_handle *h, int n_sets, const pqp_params *sets) {
         set_err("pqp_set_param_sets: bad argument (needs a handle and 1..PQP_MAX_PARAM_SETS sets)");
         return PQP_ERR_ARG;
     }
+    for (int s = 0; s < n_sets; ++s)
+        if (!settings_ok(sets[s], "pqp_set_param_sets")) return PQP_ERR_ARG;
     h->sets.assign(sets, sets + n_sets);
     h->dsets.resize((size_t)n_sets);
     for (int s = 0; s < n_sets; ++s) h->dsets[s] = pqp::dev_params_from(sets[s]);
@@ -769,6 +790,7 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
         return PQP_ERR_ARG;
     }
     *out = nullptr;
+    if (!settings_ok(*params, "pqp_create")) return PQP_ERR_ARG;
     int ndev = 0;
     PQP_CUDA(cudaGetDeviceCount(&ndev));
     if (device < 0 || device >= ndev) {

@@ -1077,7 +1077,7 @@ struct Kk {
                 const bool prim_ok = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
                 if (prim_ok && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
                 else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, 10 * pm.eps_prim_inf))
-                    status = PQP_PRIMAL_INFEASIBLE;
+                    status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
                 else status = PQP_MAX_ITER_REACHED;
             }
         }

@@ -1790,7 +1790,7 @@ struct Kp3 {
                             const bool prim_ok10 = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
                             if (prim_ok10 && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
                             else if (!prim_ok10 && primal_infeasible(c_nrm, c_lhs, c_cert, 10 * pm.eps_prim_inf))
-                                status = PQP_PRIMAL_INFEASIBLE;
+                                status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
                             else status = PQP_MAX_ITER_REACHED;
                         }
                     }

@@ -62,8 +62,11 @@ class BatchPathSolver:
             pass
 
     def set_params(self, params):
+        """Replace the parameter snapshot (pqp_set_params); settings OSQP refuses raise and leave the previous one."""
+        rc = self._L.pqp_set_params(self._h, C.byref(params))
+        if rc != OK:
+            raise PqpError(f"pqp_set_params failed (rc={rc}): {_lib.last_error()}")
         self.params = params
-        self._L.pqp_set_params(self._h, C.byref(params))
 
     def set_param_sets(self, sets):
         """Replace the parameter sets (pqp_set_param_sets): a sequence of 1..64 Params, each already run through
@@ -264,8 +267,8 @@ class OsqpSolver:
 
     def solve(self, optimized_path):
         """Fills `optimized_path` (a list) with horizon State records; returns the reference's bool."""
-        self._solver.set_params(self.params)
         try:
+            self._solver.set_params(self.params)   # (settings osqp_setup refuses fail here)
             res = self._solver.solve(self._batch, self.formulation)
         except PqpError as e:   # the reference's solve() reports every failure through its bool
             log.error("QP failed: %s", e)
