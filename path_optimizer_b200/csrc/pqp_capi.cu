@@ -1558,6 +1558,19 @@ static int solve_batch_classes(pqp_handle *h, int formulation, const int32_t *fo
                 fprintf(stderr, "[check-block cycles per path, all checks, warp %d] loads+publish x=%.0f primal=%.0f barrier=%.0f dual=%.0f certificate=%.0f reduction=%.0f\n",
                         w, ckp[0], ckp[1], ckp[2], ckp[3], ckp[4], ckp[5]);
             }
+            // refactorisation timeline: per warp and stage, the cycles until the warp reaches the stage's closing barrier
+            std::vector<long long> g4(32 * (size_t)batch), gw((size_t)batch);
+            cudaMemcpy(g4.data(), bv.debug + 48 * 65536, g4.size() * sizeof(long long), cudaMemcpyDeviceToHost);
+            cudaMemcpy(gw.data(), bv.debug + 40 * 65536, gw.size() * sizeof(long long), cudaMemcpyDeviceToHost);
+            double wsum = 0;
+            for (int b = 0; b < batch; ++b) wsum += (double)gw[b] / batch;
+            fprintf(stderr, "[refactor weights / zeroing split, thread 0] weights=%.0f zeroing+barrier=%.0f\n", wsum, rt[0] - wsum);
+            for (int w = 0; w < 4; ++w) {
+                double bz[8] = {0};
+                for (int b = 0; b < batch; ++b) for (int k = 0; k < 8; ++k) bz[k] += (double)g4[32 * (size_t)b + 8 * w + k] / batch;
+                fprintf(stderr, "[refactor busy cycles per path, warp %d] weights+zero=%.0f assembly=%.0f interior LDL=%.0f spikes=%.0f schur=%.0f block LDL=%.0f dense Sinv=%.0f dense interiors=%.0f\n",
+                        w, bz[0], bz[1], bz[2], bz[3], bz[4], bz[5], bz[6], bz[7]);
+            }
         }
     }
 #endif

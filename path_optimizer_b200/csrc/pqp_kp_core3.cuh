@@ -90,6 +90,7 @@ struct Kp3 {
     // inner loop (direct barriers, a rolled held-control loop, no integer division).  Same floating-point operations in
     // the same order, so the same bits; every other class compiles exactly as before.
     static constexpr bool kLean = IMAX == 17 && BW == 6 && NW == 4 && MMAX == 17 && FORM == 0;
+    static_assert(!kLean || (kRed2 * MMAX <= 4 * kT && (BW + 1) * MMAX <= kT), "separator scratch in exchange rows 0..3");
 
     PQP_HD static Kp3Dims dims(int N, int keep) {
         Kp3Dims d = kp3_dims_raw(N, keep, MMAX);
@@ -134,8 +135,13 @@ struct Kp3 {
         // refactorisation scratch [kRed2*M] + blocks [27*M] + couplings [12*M].  With dense interiors it lives in the
         // part of the fac / kinv region the band factor does not use (free until the dense inverses are written, which
         // is the last step of a refactorisation): two CTAs then need < 196 KB and the SM keeps 60 KB of L1 for the spills.
-        PQP_DEV double *red() const { return kDense ? fac() + IMAX * (BW + 1) * M : (kScratchOnVec ? base : Sinv() + nSd() * nSd()); }
-        PQP_DEV double *blk() const { return red() + kRed2 * M; }         // A|C|Off per chunk [27*M]
+        // The 100-station class keeps the separator-system scratch (red) in exchange rows 0..3 instead, which nothing reads
+        // from the assembly to the next iteration's (a): the dense interior inverses behind the band factor can then be
+        // built while the separator chain still reads red.
+        PQP_DEV double *red() const {
+            return kLean ? ex(0) : kDense ? fac() + IMAX * (BW + 1) * M : (kScratchOnVec ? base : Sinv() + nSd() * nSd());
+        }
+        PQP_DEV double *blk() const { return (kLean ? fac() + IMAX * (BW + 1) * M : red()) + kRed2 * M; }   // A|C|Off per chunk [27*M]
         PQP_DEV double *cpl() const { return blk() + 27 * M; }            // coupling coefs [12*M]
         // two-level form: per separator E = Dg^-1 (odd) | PL | PR (even) | Off copy [36*M]; reduced system [kRed2*ceil(M/2)]
         PQP_DEV double *lv() const { return (kDense || kScratchOnVec) ? Sinv() + nSd() * nSd() : cpl() + 12 * M; }
@@ -173,18 +179,21 @@ struct Kp3 {
     };
 
     // Dense interior inverses over the band factor (see the call site).  Out of line: what it needs in registers stays out
-    // of the solve's own allocation.
+    // of the solve's own allocation.  The 100-station class has built the rows behind the band factor already
+    // (dense_tail, during the separator block LDL'): here it solves only the staged rows.
     PQP_NOINLINE static void dense_build(const Cta &c, double *fac, int M, int tid) {
         const int Mst = M;
-        c.sync();   // the separator-system phases before it are done with the scratch behind the band factor
+        if constexpr (!kLean) c.sync();   // the separator-system phases before it are done with the scratch behind the band factor
         const int bandEnd = IMAX * (BW + 1) * M;
         const int nStaged = (bandEnd + kRow - 1) / kRow;        // <= kT for every dense class
         static_assert(!kDense || (IMAX * (BW + 1) * MMAX + kRow - 1) / kRow <= kT, "one staged row per thread");
+        if constexpr (!kLean) {
         for (int r = nStaged + tid; r < IMAX * M; r += kT) {
             const int p = r / IMAX, j = r - p * IMAX;
             double *kv = fac + (size_t)r * kRow;
             K2::local_solve_unit_mem(j, kv, fac + p, Mst);
             kv[IMAX] = 0.0;
+        }
         }
         double xc[IMAX];
         const bool staged = tid < nStaged && tid < IMAX * M;
@@ -194,6 +203,18 @@ struct Kp3 {
             double *kv = fac + (size_t)tid * kRow;
 #pragma unroll
             for (int k = 0; k < IMAX; ++k) kv[k] = xc[k];
+            kv[IMAX] = 0.0;
+        }
+    }
+    // The rows of the dense interior inverses that lie behind the band factor, solved in place: rows nStaged + t,
+    // step nt.  They read only the band factor, so they can run beside the separator chain once nothing else
+    // uses that part of the region.
+    PQP_NOINLINE static void dense_tail(double *fac, int M, int t, int nt) {
+        const int nStaged = (IMAX * (BW + 1) * M + kRow - 1) / kRow;
+        for (int r = nStaged + t; r < IMAX * M; r += nt) {
+            const int p = r / IMAX, j = r - p * IMAX;
+            double *kv = fac + (size_t)r * kRow;
+            K2::local_solve_unit_mem(j, kv, fac + p, M);
             kv[IMAX] = 0.0;
         }
     }
@@ -214,6 +235,9 @@ struct Kp3 {
         long long ph_refactor = 0, ph_check = 0, ph_scale = 0, ph_nref = 0;
         long long rt_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, rt_t = 0;
         long long ck_acc[6] = {0, 0, 0, 0, 0, 0}, ck_t = 0;   // check block (d), per warp: see PQP_CK
+        // refactorisation timeline, lane 0 of every warp: cycles from the barrier that opens stage k to the warp's arrival
+        // at the barrier that closes it (the rest of the stage the warp waits); thread 0: the row weights alone
+        long long rw_busy[8] = {0, 0, 0, 0, 0, 0, 0, 0}, rw_t = 0, rt_w = 0;
 #endif
         const int N = bv.n_points[prob];
         const int off = bv.offsets[prob];
@@ -597,13 +621,16 @@ struct Kp3 {
 
             // ================= (re)factorisation =====================================================
 #ifdef PQP_PHASE_TIMING
-#define PQP_RT(k) if (tid == 0) { const long long now_ = clock64(); rt_acc[k] += now_ - rt_t; rt_t = now_; }
+#define PQP_RT(k) { const long long now_ = clock64(); if (tid == 0) { rt_acc[k] += now_ - rt_t; rt_t = now_; } if (lane == 0) rw_t = now_; }
+#define PQP_RW(k) if (lane == 0) rw_busy[k] += clock64() - rw_t;
 #else
 #define PQP_RT(k)
+#define PQP_RW(k)
 #endif
             auto refactor = [&]() -> int {
 #ifdef PQP_PHASE_TIMING
                 if (tid == 0) rt_t = clock64();
+                if (lane == 0) rw_t = clock64();
 #endif
                 // ---- row weights W = rho_row E^2 from the workspace E
                 if (st.live) {
@@ -643,7 +670,23 @@ struct Kp3 {
                         PQP_UBW = kp_w_box(ws[oEU + tid], -kOsqpInfty, kOsqpInfty, rho);
                     }
                 }
+#ifdef PQP_PHASE_TIMING
+                if (tid == 0) rt_w += clock64() - rt_t;
+#endif
                 // zero the factor storage (identity on padded rows)
+                if constexpr (kLean) {
+                    // thread (p, dd) writes diagonal dd of chunk p, all IMAX rows: the chunk's interior size once per
+                    // thread instead of two divisions by M and two kp_gx per slot
+                    if (tid < (BW + 1) * M) {
+                        const int p = tid / (BW + 1), dd = tid - p * (BW + 1);
+                        const int g0 = kp_gx(ka, p * L);
+                        const int g1 = (p + 1 < M) ? kp_gx(ka, (p + 1) * L) : ka.nred;
+                        const int one0 = dd == 0 ? g1 - g0 - 3 : IMAX;   // padded rows from here on: 1 on the diagonal
+                        double *f = s.fac() + dd * M + p;
+#pragma unroll
+                        for (int kk = 0; kk < IMAX; ++kk) f[kk * (BW + 1) * M] = kk >= one0 ? 1.0 : 0.0;
+                    }
+                } else {
                 for (int k = tid; k < IMAX * (BW + 1) * M; k += kT) {
                     const int p = k % M, kd = k / M, dd = kd % (BW + 1), kk = kd / (BW + 1);
                     int cp = 0;
@@ -654,6 +697,8 @@ struct Kp3 {
                     }
                     s.fac()[k] = (dd == 0 && kk >= cp) ? 1.0 : 0.0;
                 }
+                }
+                PQP_RW(0)
                 c.sync();
                 PQP_RT(0)
                 // ---- assembly: every station / control thread writes its own band rows
@@ -718,6 +763,7 @@ struct Kp3 {
                     }
                     PQP_F(ku, 0) = du;
                 }
+                PQP_RW(1)
                 c.sync();
                 PQP_RT(1)
                 // ---- interior LDL' (warp 0, lane p) and coupling coefficients per chunk:
@@ -735,6 +781,7 @@ struct Kp3 {
                         cp[5] = st.WD0; cp[6] = st.WD1; cp[7] = st.WD2; cp[8] = st.dst; cp[9] = st.qt;
                     }
                 }
+                PQP_RW(2)
                 c.sync();
                 PQP_RT(2)
                 // ---- spikes: thread (p, col) solves K_I t = K[I, s_col]  (col 0..2 left, 3..5 right separator)
@@ -783,6 +830,7 @@ struct Kp3 {
                         K2::local_solve_mem(tcol, s.fac() + sp_p, Mst);   // in place in shared memory
                     }
                 }
+                PQP_RW(3)
                 c.sync();
                 PQP_RT(3)
                 // ---- Schur blocks: A_p = K[S_p,I] T_left, Off_p = -(K[S_q,I] T_left)', C_p = K[S_q,I] T_right
@@ -835,6 +883,7 @@ struct Kp3 {
                         for (int k = 0; k < 9; ++k) s.lv()[36 * p + 27 + k] = B[18 + k];   // Off_p = S[p, p+1]
                     }
                 }
+                PQP_RW(4)
                 c.sync();
                 if constexpr (kTwoLevel) {
                     // ---- level 1: odd separators are eliminated.  E_p = Dg_p^-1 (p odd); for even p
@@ -939,6 +988,13 @@ struct Kp3 {
                         for (int k = 0; k < 9; ++k) Rp[k] = Sinv[k];
                     }
                 }
+                // 100-station class: meanwhile warps 1.. build the dense interior rows behind the band factor.  The
+                // separator scratch is not there (red() is in the exchange rows), and the spikes and Schur blocks, the
+                // last readers of the rest of that region, are done.
+                if constexpr (kLean) {
+                    if (wid > 0) dense_tail(s.fac(), M, tid - 32, kT - 32);
+                }
+                PQP_RW(5)
                 c.sync();
                 PQP_RT(5)
                 // ---- dense inverse of the separator system: thread t solves for unit vector e_t and
@@ -973,6 +1029,7 @@ struct Kp3 {
                         x0 = y0; x1 = y1; x2 = y2;
                     }
                 }
+                PQP_RW(6)
                 PQP_RT(6)
                 if constexpr (kDense) {
                     // ---- dense interior inverses, row-major over the band factor: row r = p * IMAX + j of the
@@ -982,6 +1039,7 @@ struct Kp3 {
                     //      in registers and written once everybody is done.
                     dense_build(c, s.fac(), M, tid);
                 }
+                PQP_RW(7)
                 PQP_RT(7)
                 if constexpr (kScratchOnVec) {
                     c.sync();   // every reader of the scratch is done: give the two vectors back, padded entries zero
@@ -1742,17 +1800,48 @@ struct Kp3 {
                         // the 14 maxima and (checks only) the certificate's sum u'g+ + l'g- over the CTA in ONE shared
                         // exchange: warp butterflies, one slot row of 16 per warp, and the cross-warp combine unrolled
                         // over the compile-time warp count.  Same operations in the same order as Cta::max_n and
-                        // Cta::sum (warp 0's partial first, then warps 1, 2, ...), so the same bits.
+                        // Cta::sum (warp 0's partial first, then warps 1, 2, ...), so the same bits; the 100-station
+                        // class reduces the maxima inside a warp in another order, which gives the same bits too.
                         double red[14] = {pr, nz, nax, prs, nzs, naxs, dr, npx, naty, drs, npxs, natys, c_nrm, c_cert};
                         static_assert(NW > 1 && 16 * NW <= kCtaScratch, "one slot row of 16 per warp");
+                        double *const sc = c.scratch;
+                        if constexpr (kLean) {
+                            // 100-station class: each of the 14 is a maximum of magnitudes (fabs, or fabs times a positive
+                            // scaling, starting from +0), so fmax gives the same bits in any order: a NaN is dropped
+                            // unless all are NaN, and then only its NaN-ness is read.  The warp step is a transposed
+                            // reduction instead of 14 butterflies: at xor distance o a lane keeps one half of its
+                            // values and trades the other half with lane ^ o, 16 shuffles instead of 70, and lane 2k
+                            // ends with value k.  The certificate's sum keeps its butterfly (its order matters).
+                            double v[16];
+#pragma unroll
+                            for (int k = 0; k < 14; ++k) v[k] = red[k];
+                            v[14] = 0.0; v[15] = 0.0;
+                            auto half = [&](auto n_) {   // xor distance 2 n: keep n values, trade n
+                                constexpr int n = decltype(n_)::value;
+                                const bool hi = (lane & (2 * n)) != 0;
+#pragma unroll
+                                for (int j = 0; j < n; ++j) {
+                                    const double keep = hi ? v[n + j] : v[j], give = hi ? v[j] : v[n + j];
+                                    v[j] = fmax(keep, c.w.shfl(give, lane ^ (2 * n)));
+                                }
+                            };
+                            half(std::integral_constant<int, 8>{});
+                            half(std::integral_constant<int, 4>{});
+                            half(std::integral_constant<int, 2>{});
+                            half(std::integral_constant<int, 1>{});
+                            const double x = fmax(v[0], c.w.shfl(v[0], lane ^ 1));
+                            if (chk) c_lhs = c.w.sum(c_lhs);
+                            if (!(lane & 1) && lane < 28) sc[wid * 16 + (lane >> 1)] = x;
+                            if (lane == 0) sc[wid * 16 + 14] = c_lhs;
+                        } else {
 #pragma unroll
                         for (int k = 0; k < 14; ++k) red[k] = c.w.max(red[k]);
                         if (chk) c_lhs = c.w.sum(c_lhs);
-                        double *const sc = c.scratch;
                         if (lane == 0) {
 #pragma unroll
                             for (int k = 0; k < 14; ++k) sc[wid * 16 + k] = red[k];
                             sc[wid * 16 + 14] = c_lhs;
+                        }
                         }
                         c.cs.sync();
 #pragma unroll
@@ -1900,6 +1989,9 @@ struct Kp3 {
         if (kPhTime && bv.debug && lane == 0 && wid < 4 && status != PQP_INVALID_PROBLEM) {
             long long *g3 = bv.debug + 32 * 65536 + 32 * (size_t)prob + 8 * wid;
             for (int k = 0; k < 6; ++k) g3[k] = ck_acc[k];
+            long long *g4 = bv.debug + 48 * 65536 + 32 * (size_t)prob + 8 * wid;
+            for (int k = 0; k < 8; ++k) g4[k] = rw_busy[k];
+            if (wid == 0) bv.debug[40 * 65536 + (size_t)prob] = rt_w;
         }
 #endif
         // ---- epilogue: getOptimizedPath, solver_kp_as_input.cpp:26-43
