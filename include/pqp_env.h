@@ -160,6 +160,63 @@ int pqp_spline_fit(int n, const double *t, const double *y, double *coef /* [n][
 int pqp_fit_splines_device(pqp_handle *h, int batch, int total_points, const int32_t *d_offsets, const pqp_state *d_ref,
                            double *d_knots, double *d_x_coef, double *d_y_coef, int32_t *d_ok, void *stream);
 
+/* Segment smoothed reference lines into reference states for every path of a batch, on DEVICE arrays of the handle's
+ * device: what segmentSmoothedPath (path_optimizer.cpp:119-178) does between the smoother and the QP, with outputs in
+ * the layout pqp_plan_batch_device* takes.
+ *   d_knot_offsets, d_knots, d_x_coef, d_y_coef   every path's x(s), y(s) splines, the layout pqp_fit_splines_device
+ *                      writes and pqp_plan_batch_device* reads with PQP_BOUNDS_IMPROVED
+ *   d_max_s            [batch] every line's length, what ReferencePathImpl::setSpline receives
+ *   d_start, d_goal    [batch] VehicleState's start and end states
+ *   delta_s_smaller, delta_s_larger   the spacings of :168-173: (0.15, FLAGS_output_spacing) with
+ *                      FLAGS_enable_raw_output, else (0.5, 1.0)
+ *   dynamic_segmentation   FLAGS_enable_dynamic_segmentation
+ *   search_delta_s     the goal-search step: 0.1 with FLAGS_enable_exact_position, else 0.5
+ *   max_n_points       stations a path may have at most
+ *   capacity           stations d_ref holds (the total_points to plan with)
+ *   d_n_points         [batch] out: stations of every path (0 when refused)
+ *   d_offsets          [batch+1] out: their exclusive prefix; d_offsets[batch] <= capacity (with batch = 0 the
+ *                      one entry 0 is written when d_offsets is not NULL)
+ *   d_ref              [capacity] out: the stations, x, y, z, k, s filled, v = a = 0; entries past d_offsets[batch]
+ *                      are not written
+ *   d_x0               [batch][3] out: (initial offset, initial heading error, start.k), written for every path
+ *   d_end_heading      [batch] out: goal.z
+ *   d_ok               [batch] out: 1 when the path was segmented, 0 when it was refused
+ * Per path: the initial offset is the distance from the start to the spline's first point, positive when that point
+ * lies right of the start's heading, and the heading error constraintAngle(start.z - heading at s = 0) (:125-141);
+ * when the goal is not within 1e-6 of the point at max_s, the length is cut to the sample closest to the goal on the
+ * lattice max_s - i * search_delta_s (accumulated), searched backwards until a sample lies more than 8 m from the goal
+ * while the closest lies within 8 m (:143-166); then ReferencePathImpl::buildReferenceFromSpline (reference_path_impl.cpp
+ * :474-499) samples s = 0, s1, ... <= the cut length, each step delta_s_larger, or with dynamic segmentation shortened
+ * towards delta_s_smaller as |k| goes from 0.08 to 0.2.  Heading and curvature come from the splines' derivatives as
+ * getHeading and getCurvature compute them (tools.cpp:32-44), in the arithmetic of the densifying tail.
+ * A path is refused (ok = 0, 0 stations; no other path changes) when:
+ *   - its splines have fewer than 3 knots, its initial offset is not finite, or start.z minus the heading at s = 0 is
+ *     not finite or exceeds 2^20 rad in magnitude (e.g. the NaN rows of a line pqp_fit_splines_device refused, or a
+ *     NaN start);
+ *   - |initial heading error| > 75 degrees (:137-140);
+ *   - max_s <= 0 or is not finite, or max_s > search_delta_s * 2^22 (a goal search too long to walk).  The guard
+ *     still admits long searches: a goal that is NaN or more than 8 m from every sample visits every lattice sample,
+ *     about 1.1 us each on one thread of an H100, so up to about 4.6 s for one path at the limit;
+ *   - it needs more than max_n_points stations;
+ *   - the running total of stations, in index order, would pass capacity: path b is refused when the stations of paths
+ *     0..b, refused ones counting 0, exceed capacity, and so is every later path with stations.
+ * To fail a refused path in the plan without a host round trip, give it a map index outside the map set on the device
+ * (map_index[b] = d_ok[b] ? map_index[b] : -1), as for pqp_fit_splines_device.
+ * NULL pointers (with batch > 0), a negative batch or capacity, max_n_points < 1, or spacings that are not positive and
+ * finite or with delta_s_larger < delta_s_smaller return PQP_ERR_ARG; a batch above the handle's max_batch or a
+ * capacity above its max_total_points PQP_ERR_CAPACITY; nothing is launched then.  Asynchronous on `stream` (NULL: the
+ * handle's stream), no host synchronisation; the scratch (one int32 per path of the handle's max_batch) is allocated by
+ * the first call, after which the call allocates nothing and can be captured in a CUDA graph between
+ * pqp_fit_splines_device and the plan entries.  No map set is needed.
+ * Replaces: PathOptimizer::segmentSmoothedPath (path_optimizer.cpp:119-173) up to buildReferenceFromSpline, once per
+ * path; the bounds and limits it goes on to compute are the plan entries' stages. */
+int pqp_segment_reference_device(pqp_handle *h, int batch, const int32_t *d_knot_offsets, const double *d_knots,
+                                 const double *d_x_coef, const double *d_y_coef, const double *d_max_s,
+                                 const pqp_state *d_start, const pqp_state *d_goal, double delta_s_smaller,
+                                 double delta_s_larger, int dynamic_segmentation, double search_delta_s,
+                                 int max_n_points, int capacity, int32_t *d_n_points, int32_t *d_offsets,
+                                 pqp_state *d_ref, double *d_x0, double *d_end_heading, int32_t *d_ok, void *stream);
+
 /* tk::spline::operator() / deriv (spline.cpp:250-318) on a fitted spline; order 0..2. */
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at);
 

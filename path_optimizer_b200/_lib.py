@@ -20,7 +20,8 @@ ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "
                "pqp_check_states", "pqp_finish_raw_batch", "pqp_densify_batch", "pqp_plan_batch", "pqp_plan_batch_device",
                "pqp_set_maps", "pqp_plan_batch_maps", "pqp_plan_batch_device_maps", "pqp_plan_batch_sets",
                "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map",
-               "pqp_plan_batch_forms", "pqp_plan_batch_device_forms", "pqp_fit_splines_device"]
+               "pqp_plan_batch_forms", "pqp_plan_batch_device_forms", "pqp_fit_splines_device",
+               "pqp_segment_reference_device"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -102,6 +103,8 @@ def load():
     L.pqp_set_maps_occupancy_device.argtypes = [vp, C.c_int, C.POINTER(OccupancyMap), vp]
     L.pqp_get_map.argtypes = [vp, C.c_int, vp]
     L.pqp_fit_splines_device.argtypes = [vp, C.c_int, C.c_int] + [vp] * 7
+    L.pqp_segment_reference_device.argtypes = ([vp, C.c_int] + [vp] * 7 + [C.c_double, C.c_double, C.c_int, C.c_double,
+                                                C.c_int, C.c_int] + [vp] * 7)
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

@@ -16,6 +16,7 @@
 
 #include "pqp_edt_core.cuh"
 #include "pqp_env_core.cuh"
+#include "pqp_segment_core.cuh"
 #include "pqp_dispatch.h"
 #include "pqp_handle.h"
 
@@ -57,6 +58,8 @@ struct EnvState {
     size_t knot_cap = 0;
     // pqp_fit_splines_device: diag and rhs of both coordinates, 4 doubles per station (max_total, at first use)
     double *d_fit = nullptr;
+    // pqp_segment_reference_device: every path's station count between its launches (max_batch, at first use)
+    int32_t *d_seg = nullptr;
     // generic scratch for pqp_map_distance / pqp_check_states (grow-only)
     char *d_tmp = nullptr;
     size_t tmp_cap = 0;
@@ -68,7 +71,7 @@ void env_free(void *p) {
     cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx); cudaFree(e->d_setidx);
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
-    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit);
+    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit); cudaFree(e->d_seg);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     delete e;
 }
@@ -403,6 +406,88 @@ pqp_fit_splines_kernel(const __grid_constant__ FitArgs a) {
     const size_t o = (size_t)off;
     pqp::fit_path_coord(max(n, 0), ok, coord, a.ref + o, a.knots + o, (coord ? a.yc : a.xc) + 4 * o, a.scr + 4 * o);
     if (coord == 0) a.ok[b] = ok ? 1 : 0;
+}
+
+// pqp_segment_reference_device: three launches on the caller's stream.  (1) one thread per path walks its line once to
+// count its stations (pqp::segment_count) and writes x0 and end_heading; (2) one warp reserves the stations in index
+// order and writes n_points, offsets and ok; (3) one thread per kept path walks its line again and writes its states
+// (pqp::segment_write), the same samples bit for bit.  The counts sit in the handle's scratch between the launches.
+struct SegmentArgs {
+    pqp::SegmentFlags f;
+    int batch;
+    long long capacity;
+    const int32_t *koff;
+    const double *knots, *xc, *yc;
+    const double *max_s;
+    const pqp_state *start, *goal;
+    int32_t *count;          // scratch [batch]: stations of every path, 0 when refused
+    int32_t *n_points, *offsets, *ok;
+    pqp_state *ref;
+    double *x0, *end_heading;
+};
+constexpr int kSegmentThreads = 128;
+
+__device__ __forceinline__ void segment_splines(const SegmentArgs &a, int b, SplineView &xs, SplineView &ys) {
+    const int o = a.koff[b], n = a.koff[b + 1] - o;
+    xs = SplineView{n, a.knots + o, a.xc + 4 * (size_t)o};
+    ys = SplineView{n, a.knots + o, a.yc + 4 * (size_t)o};
+}
+
+__global__ void __launch_bounds__(kSegmentThreads)
+pqp_segment_count_kernel(const __grid_constant__ SegmentArgs a) {
+    const int b = blockIdx.x * kSegmentThreads + threadIdx.x;
+    if (b >= a.batch) return;
+    SplineView xs, ys;
+    segment_splines(a, b, xs, ys);
+    const pqp_state start = a.start[b], goal = a.goal[b];
+    double x0[3], cut_s;
+    int n;
+    pqp::segment_count(a.f, xs, ys, a.max_s[b], start, goal, x0, &cut_s, &n);
+    a.count[b] = n;
+    a.x0[3 * (size_t)b + 0] = x0[0];
+    a.x0[3 * (size_t)b + 1] = x0[1];
+    a.x0[3 * (size_t)b + 2] = x0[2];
+    a.end_heading[b] = goal.z;
+}
+
+__device__ __forceinline__ long long warp_inclusive_sum(long long v) {
+    const int lane = threadIdx.x & 31;
+    for (int d = 1; d < 32; d <<= 1) {
+        const long long u = __shfl_up_sync(0xffffffffu, v, d);
+        if (lane >= d) v += u;
+    }
+    return v;
+}
+
+__global__ void __launch_bounds__(32)
+pqp_segment_scan_kernel(const __grid_constant__ SegmentArgs a) {
+    const int lane = threadIdx.x;
+    long long all = 0, kept = 0;      // stations of every path before the tile, and of the kept ones
+    if (lane == 0) a.offsets[0] = 0;
+    for (int b0 = 0; b0 < a.batch; b0 += 32) {
+        const int b = b0 + lane;
+        const int c = b < a.batch ? a.count[b] : 0;
+        const long long ia = warp_inclusive_sum(c);
+        const bool keep = pqp::segment_fits(all + ia - c, c, a.capacity);
+        const int ck = keep ? c : 0;
+        const long long ik = warp_inclusive_sum(ck);
+        if (b < a.batch) {
+            a.n_points[b] = ck;
+            a.offsets[b + 1] = (int32_t)(kept + ik);
+            a.ok[b] = keep ? 1 : 0;
+        }
+        all += __shfl_sync(0xffffffffu, ia, 31);
+        kept += __shfl_sync(0xffffffffu, ik, 31);
+    }
+}
+
+__global__ void __launch_bounds__(kSegmentThreads)
+pqp_segment_write_kernel(const __grid_constant__ SegmentArgs a) {
+    const int b = blockIdx.x * kSegmentThreads + threadIdx.x;
+    if (b >= a.batch || !a.ok[b]) return;
+    SplineView xs, ys;
+    segment_splines(a, b, xs, ys);
+    pqp::segment_write(a.f, xs, ys, a.n_points[b], a.ref + a.offsets[b]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -848,6 +933,50 @@ int pqp_fit_splines_device(pqp_handle *h, int batch, int total_points, const int
     cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
     const FitArgs a{batch, d_offsets, d_ref, d_knots, d_x_coef, d_y_coef, e->d_fit, d_ok};
     pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    return PQP_OK;
+}
+
+int pqp_segment_reference_device(pqp_handle *h, int batch, const int32_t *d_knot_offsets, const double *d_knots,
+                                 const double *d_x_coef, const double *d_y_coef, const double *d_max_s,
+                                 const pqp_state *d_start, const pqp_state *d_goal, double delta_s_smaller,
+                                 double delta_s_larger, int dynamic_segmentation, double search_delta_s,
+                                 int max_n_points, int capacity, int32_t *d_n_points, int32_t *d_offsets,
+                                 pqp_state *d_ref, double *d_x0, double *d_end_heading, int32_t *d_ok, void *stream) {
+    const bool spacing_ok = delta_s_smaller > 0 && delta_s_larger >= delta_s_smaller && isfinite(delta_s_larger) &&
+                            search_delta_s > 0 && isfinite(search_delta_s);
+    if (!h || batch < 0 || capacity < 0 || max_n_points < 1 || !spacing_ok ||
+        (batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef || !d_max_s || !d_start || !d_goal ||
+                       !d_n_points || !d_offsets || !d_ref || !d_x0 || !d_end_heading || !d_ok))) {
+        pqp_set_err("pqp_segment_reference_device: bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (batch > h->max_batch || capacity > h->max_total) {
+        pqp_set_err("batch / capacity exceed what the handle was created for (max_batch, max_total_points)");
+        return PQP_ERR_CAPACITY;
+    }
+    EnvState *e;
+    int rc = env_get(h, &e);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    if (batch == 0) {                     // an empty batch still gets offsets[0] = 0 when the array is given
+        if (d_offsets) PQP_CUDA(cudaMemsetAsync(d_offsets, 0, sizeof(int32_t), st));
+        return PQP_OK;
+    }
+    if (!e->d_seg) PQP_CUDA(cudaMalloc(&e->d_seg, (size_t)h->max_batch * sizeof(int32_t)));
+    SegmentArgs a;
+    a.f = pqp::SegmentFlags{delta_s_smaller, delta_s_larger, search_delta_s, dynamic_segmentation ? 1 : 0, max_n_points};
+    a.batch = batch; a.capacity = capacity;
+    a.koff = d_knot_offsets; a.knots = d_knots; a.xc = d_x_coef; a.yc = d_y_coef;
+    a.max_s = d_max_s; a.start = d_start; a.goal = d_goal; a.count = e->d_seg;
+    a.n_points = d_n_points; a.offsets = d_offsets; a.ok = d_ok; a.ref = d_ref; a.x0 = d_x0; a.end_heading = d_end_heading;
+    const int grid = (batch + kSegmentThreads - 1) / kSegmentThreads;
+    pqp_segment_count_kernel<<<grid, kSegmentThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    pqp_segment_scan_kernel<<<1, 32, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    pqp_segment_write_kernel<<<grid, kSegmentThreads, 0, st>>>(a);
     PQP_CUDA(cudaGetLastError());
     return PQP_OK;
 }

@@ -6,6 +6,7 @@ Reference interfaces being mirrored:
   CollisionChecker::isSingleStateCollisionFreeImproved   src/tools/collision_checker.cpp:41-59
   PathOptimizer::optimizePath tails                      src/path_optimizer/path_optimizer.cpp:191-230
   PathOptimizer::solveWithoutSmoothing                   src/path_optimizer/path_optimizer.cpp:87-117
+  PathOptimizer::segmentSmoothedPath                     src/path_optimizer/path_optimizer.cpp:119-178
   tk::spline set_points / operator() / deriv             src/tools/spline.cpp:161-318
 
 All numerics run in libpqp.so's sm_90a kernels (spline_fit / spline_eval are host helpers of the
@@ -298,6 +299,48 @@ class PathPlanner(BatchPathSolver):
         if rc != OK:
             raise PqpError(f"pqp_fit_splines_device failed (rc={rc}): {_lib.last_error()}")
         return dict(knot_offsets=offsets, knots=knots, x_coef=xc, y_coef=yc, ok=ok)
+
+    def segment_device(self, splines, max_s, start, goal, max_n_points, capacity=None, delta_s_smaller=0.15,
+                       delta_s_larger=0.3, dynamic_segmentation=True, search_delta_s=0.5, out=None):
+        """PathOptimizer::segmentSmoothedPath for every path of a batch on the device (pqp_segment_reference_device):
+        smoothed lines in, the reference states plan_device reads out.  `splines` a dict of knot_offsets int32 [B + 1],
+        knots [K], x_coef / y_coef [K, 4] (fit_splines_device's output or device.splines_to_device), max_s float64 [B]
+        the lines' lengths, start / goal float64 [B, 7] states, all torch CUDA tensors; on torch.cuda.current_stream().
+        The defaults are the reference's flags: raw output with output_spacing 0.3 (spacings 0.15 and 0.3; without raw
+        output 0.5 and 1.0), dynamic segmentation on, exact position off (search step 0.5; 0.1 with it).  capacity:
+        stations the output holds (default the planner's max_total_points), the total_points to plan with.
+        Returns dict(n_points int32 [B], offsets int32 [B + 1], ref float64 [capacity, 7], x0 [B, 3], end_heading [B],
+        ok int32 [B]).  A refused path (heading error over 75 degrees, max_s <= 0 or not finite, more than
+        max_n_points stations, past the capacity in index order, or a spline that is not usable) gets ok = 0 and 0
+        stations; fail it in plan_device with map_index = torch.where(ok != 0, map_index, -1).  No host
+        synchronisation; after one call on the planner it can be captured in a CUDA graph.  `out` may carry the output
+        tensors, e.g. those of an earlier call, so that a captured graph writes where the plan reads."""
+        import torch
+        from . import device as D
+        dev = self._cuda_device()
+        B = int(max_s.shape[0])
+        cap = int(self.max_total_points if capacity is None else capacity)
+        K = int(splines["knots"].shape[0])
+        f64, i32 = torch.float64, torch.int32
+        out = dict(out or {})
+
+        def buf(name, shp, dtype):
+            return out[name] if out.get(name) is not None else torch.empty(shp, dtype=dtype, device=dev)
+        n_points, offsets, ok = buf("n_points", (B,), i32), buf("offsets", (B + 1,), i32), buf("ok", (B,), i32)
+        ref, x0, end_heading = buf("ref", (cap, D.STATE_COLS), f64), buf("x0", (B, 3), f64), buf("end_heading", (B,), f64)
+        rc = self._L.pqp_segment_reference_device(
+            self._h, B, D.check(splines["knot_offsets"], "knot_offsets", i32, (B + 1,), dev),
+            D.check(splines["knots"], "knots", f64, (K,), dev), D.check(splines["x_coef"], "x_coef", f64, (K, 4), dev),
+            D.check(splines["y_coef"], "y_coef", f64, (K, 4), dev), D.check(max_s, "max_s", f64, (B,), dev),
+            D.check(start, "start", f64, (B, D.STATE_COLS), dev), D.check(goal, "goal", f64, (B, D.STATE_COLS), dev),
+            float(delta_s_smaller), float(delta_s_larger), int(bool(dynamic_segmentation)), float(search_delta_s),
+            int(max_n_points), cap, D.check(n_points, "n_points", i32, (B,), dev),
+            D.check(offsets, "offsets", i32, (B + 1,), dev), D.check(ref, "ref", f64, (cap, D.STATE_COLS), dev),
+            D.check(x0, "x0", f64, (B, 3), dev), D.check(end_heading, "end_heading", f64, (B,), dev),
+            D.check(ok, "ok", i32, (B,), dev), torch.cuda.current_stream(dev).cuda_stream)
+        if rc != OK:
+            raise PqpError(f"pqp_segment_reference_device failed (rc={rc}): {_lib.last_error()}")
+        return dict(n_points=n_points, offsets=offsets, ref=ref, x0=x0, end_heading=end_heading, ok=ok)
 
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
