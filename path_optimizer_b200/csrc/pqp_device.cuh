@@ -115,4 +115,74 @@ PQP_DEV bool primal_infeasible(double nrm, double lhs, double cert, double eps) 
     return nrm > eps && lhs < -eps * nrm && cert < eps * nrm;
 }
 
+// What a termination check compares, in unscaled terms: the primal and dual residuals with the norms
+// their relative tolerances scale, and the primal-infeasibility certificate of primal_infeasible.
+struct Residuals {
+    double pri_res, dua_res, pri_nrm, dua_nrm;
+    double inf_nrm, inf_lhs, inf_cert;
+};
+
+// OSQP check_termination (unscaled residuals, strict <): PQP_NON_CVX, PQP_SOLVED,
+// PQP_PRIMAL_INFEASIBLE or PQP_UNSOLVED.  q = 0, so the dual-infeasibility test (q'dx < 0) never fires.
+PQP_DEV int termination_verdict(const DevParams &pm, const Residuals &r) {
+    const bool prim_ok = r.pri_res < pm.eps_abs + pm.eps_rel * r.pri_nrm;
+    if (r.pri_res > kOsqpInfty || r.dua_res > kOsqpInfty) return PQP_NON_CVX;
+    if (prim_ok && r.dua_res < pm.eps_abs + pm.eps_rel * r.dua_nrm) return PQP_SOLVED;
+    if (!prim_ok && primal_infeasible(r.inf_nrm, r.inf_lhs, r.inf_cert, pm.eps_prim_inf)) return PQP_PRIMAL_INFEASIBLE;
+    return PQP_UNSOLVED;
+}
+
+// max_iter reached without a verdict: OSQP re-checks the last residuals with 10x tolerances.
+PQP_DEV int max_iter_verdict(const DevParams &pm, const Residuals &r) {
+    const bool prim_ok = r.pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * r.pri_nrm;
+    if (prim_ok && r.dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * r.dua_nrm) return PQP_SOLVED_INACCURATE;
+    if (!prim_ok && primal_infeasible(r.inf_nrm, r.inf_lhs, r.inf_cert, 10 * pm.eps_prim_inf))
+        return PQP_PRIMAL_INFEASIBLE_INACCURATE;
+    return PQP_MAX_ITER_REACHED;
+}
+
+// OSQP compute_rho_estimate on the SCALED residuals and norms (in the order of Residuals), clamped to
+// [kRhoMin, kRhoMax].
+PQP_DEV double rho_estimate(double rho, double pri_res, double dua_res, double pri_nrm, double dua_nrm) {
+    const double pn = pri_res / (pri_nrm + 1e-10);
+    const double dn = dua_res / (dua_nrm + 1e-10);
+    const double rho_new = rho * sqrt(pn / (dn + 1e-10));
+    return fmin(fmax(rho_new, kRhoMin), kRhoMax);
+}
+
+// OSQP adapts rho only when the estimate leaves [rho / tol, rho * tol], tol = adaptive_rho_tolerance.
+// `|` rather than `||` is a code-generation choice: both compares (and rho / tol) are evaluated; with `||`
+// the "K" and "KPC" kernels spill more.  The outcome is the same.
+PQP_DEV bool rho_changed(const DevParams &pm, double rho_new, double rho) {
+    const double tol = pm.adaptive_rho_tolerance;
+    return (rho_new > rho * tol) | (rho_new < rho / tol);
+}
+
+// The statuses whose iterate the solver returns (OSQP's solution is kept at max_iter too).
+PQP_DEV bool has_solution(int status) {
+    return status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED;
+}
+
+// One station of getOptimizedPath (solver_kp_as_input.cpp:26-43): the point at lateral offset ey from the
+// reference state r, with heading r.z + ephi and curvature kk.  Writes every field of o but the arc length;
+// (tx, ty) is the point, for the arc-length pass.  The cores store their scratch copies of (tx, ty) next,
+// then call store_frenet.
+PQP_DEV void optimized_station(const pqp_state &r, double ey, double ephi, double kk, pqp_state &o,
+                               double &tx, double &ty) {
+    const double angle = r.z;
+    const double new_angle = constraint_angle(angle + 1.57079632679489661923);
+    tx = r.x + ey * cos(new_angle);
+    ty = r.y + ey * sin(new_angle);
+    o.x = tx; o.y = ty; o.z = angle + ephi; o.k = kk;
+    o.v = 0.0; o.a = 0.0;
+}
+
+// The Frenet triple (e_y, e_phi, kappa) of station k, when out_frenet is set.
+PQP_DEV void store_frenet(double *out_frenet, int k, double ey, double ephi, double kk) {
+    if (out_frenet) {
+        double *f = out_frenet + 3 * (size_t)k;
+        f[0] = ey; f[1] = ephi; f[2] = kk;
+    }
+}
+
 }  // namespace pqp

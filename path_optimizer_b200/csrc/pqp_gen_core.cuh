@@ -358,8 +358,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         w.sync();
         if (!gen_factor(w, cx, cost_c)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
-        double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
-        double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;   // primal-infeasibility certificate of the last check
+        Residuals res{};   // of the last check
         iter = 0;
         while (status == PQP_UNSOLVED && iter < pm.max_iter) {
             ++iter;
@@ -445,24 +444,14 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                         for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) aty += cx.csc_val[e] * cx.wold[cx.csc_row[e]];
                         c_cert = fmax(c_cert, fabs(aty));
                     }
-                    inf_nrm = w.max(c_nrm); inf_cert = w.max(c_cert); inf_lhs = w.sum(c_lhs);
+                    res.inf_nrm = w.max(c_nrm); res.inf_cert = w.max(c_cert); res.inf_lhs = w.sum(c_lhs);
                     w.sync();
                 }
-                pri_res = pr; dua_res = dr; pri_nrm = fmax(nz, nax); dua_nrm = fmax(npx, naty);
-                if (can_check || iter == pm.max_iter) {
-                    // OSQP check_termination; q = 0, so the dual-infeasibility test (q'dx < 0) never fires
-                    const bool prim_ok = pri_res < pm.eps_abs + pm.eps_rel * pri_nrm;
-                    if (pri_res > kOsqpInfty || dua_res > kOsqpInfty) status = PQP_NON_CVX;
-                    else if (prim_ok && dua_res < pm.eps_abs + pm.eps_rel * dua_nrm) status = PQP_SOLVED;
-                    else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, pm.eps_prim_inf))
-                        status = PQP_PRIMAL_INFEASIBLE;
-                }
+                res.pri_res = pr; res.dua_res = dr; res.pri_nrm = fmax(nz, nax); res.dua_nrm = fmax(npx, naty);
+                if (can_check || iter == pm.max_iter) status = termination_verdict(pm, res);
                 if (status == PQP_UNSOLVED && can_adapt) {
-                    const double pn = prs / (fmax(nzs, naxs) + 1e-10);
-                    const double dn = drs / (fmax(npxs, natys) + 1e-10);
-                    double rho_new = rho * sqrt(pn / (dn + 1e-10));
-                    rho_new = fmin(fmax(rho_new, kRhoMin), kRhoMax);
-                    if (rho_new > rho * pm.adaptive_rho_tolerance || rho_new < rho / pm.adaptive_rho_tolerance) {
+                    const double rho_new = rho_estimate(rho, prs, drs, fmax(nzs, naxs), fmax(npxs, natys));
+                    if (rho_changed(pm, rho_new, rho)) {
                         for (int r = lane; r < m; r += 32) {
                             const double El = cx.E[r] * cx.l[r], Eu = cx.E[r] * cx.u[r];
                             const double ro = rho_bar(El, Eu, rho), rn = rho_bar(El, Eu, rho_new);
@@ -477,32 +466,20 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                 }
             }
         }
-        if (status == PQP_UNSOLVED) {
-            const bool prim_ok = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
-            if (prim_ok && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
-            else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, 10 * pm.eps_prim_inf))
-                status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
-            else status = PQP_MAX_ITER_REACHED;
-        }
+        if (status == PQP_UNSOLVED) status = max_iter_verdict(pm, res);
     }
     // ---- epilogue: getOptimizedPath (solver_k_as_input.cpp:22-44, ..._constrained.cpp:26-43)
-    const bool has_sol = (status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED);
+    const bool has_sol = has_solution(status);
     const int32_t *oi = gv.out_idx + 3 * (size_t)offN;
     w.sync();
     double *px = bad ? nullptr : cx.tr, *py = bad ? nullptr : cx.tmp;
     for (int i = lane; i < N; i += 32) {
-        double ey = qnan, ephi = qnan, kk = qnan;
+        double ey = qnan, ephi = qnan, kk = qnan, tx, ty;
         if (has_sol) { ey = cx.xr[oi[3 * i]]; ephi = cx.xr[oi[3 * i + 1]]; kk = cx.xr[oi[3 * i + 2]]; }
-        const double angle = ref[i].z;
-        const double new_angle = constraint_angle(angle + 1.57079632679489661923);
-        const double tx = ref[i].x + ey * cos(new_angle), ty = ref[i].y + ey * sin(new_angle);
-        out[i].x = tx; out[i].y = ty; out[i].z = angle + ephi; out[i].k = kk; out[i].v = 0.0; out[i].a = 0.0;
+        optimized_station(ref[i], ey, ephi, kk, out[i], tx, ty);
         out[i].s = qnan;
         if (px) { px[i] = tx; py[i] = ty; }
-        if (gv.out_frenet) {
-            double *f = gv.out_frenet + 3 * (size_t)(offN + i);
-            f[0] = ey; f[1] = ephi; f[2] = kk;
-        }
+        store_frenet(gv.out_frenet, offN + i, ey, ephi, kk);
     }
     w.sync();
     if (lane == 0) {

@@ -910,8 +910,7 @@ struct Kk {
             if (c.any(split)) status = PQP_INVALID_PROBLEM;
             else if (!factor()) status = PQP_NON_CVX;
             const double alpha = pm.alpha;
-            double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
-            double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;
+            Residuals res{};
             iter = 0;
             // (iter % interval == 0 without a division per iteration: the next multiple is tracked)
             const int ct = pm.check_termination, ai = (pm.adaptive_rho ? pm.adaptive_rho_interval : 0);
@@ -1038,23 +1037,14 @@ struct Kk {
                         }
                         double r2[2] = {c_nrm, c_cert};
                         c.max_n(r2, 2);
-                        inf_nrm = r2[0]; inf_cert = r2[1];
-                        inf_lhs = c.sum(c_lhs);
+                        res.inf_nrm = r2[0]; res.inf_cert = r2[1];
+                        res.inf_lhs = c.sum(c_lhs);
                     }
-                    pri_res = pr; dua_res = dr; pri_nrm = fmax(nz, nax); dua_nrm = fmax(npx, naty);
-                    if (can_check || iter == pm.max_iter) {
-                        const bool prim_ok = pri_res < pm.eps_abs + pm.eps_rel * pri_nrm;
-                        if (pri_res > kOsqpInfty || dua_res > kOsqpInfty) status = PQP_NON_CVX;
-                        else if (prim_ok && dua_res < pm.eps_abs + pm.eps_rel * dua_nrm) status = PQP_SOLVED;
-                        else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, pm.eps_prim_inf))
-                            status = PQP_PRIMAL_INFEASIBLE;
-                    }
+                    res.pri_res = pr; res.dua_res = dr; res.pri_nrm = fmax(nz, nax); res.dua_nrm = fmax(npx, naty);
+                    if (can_check || iter == pm.max_iter) status = termination_verdict(pm, res);
                     if (status == PQP_UNSOLVED && can_adapt) {
-                        const double pn = prs / (fmax(nzs, naxs) + 1e-10);
-                        const double dn = drs / (fmax(npxs, natys) + 1e-10);
-                        double rho_new = rho * sqrt(pn / (dn + 1e-10));
-                        rho_new = fmin(fmax(rho_new, kRhoMin), kRhoMax);
-                        if (rho_new > rho * pm.adaptive_rho_tolerance || rho_new < rho / pm.adaptive_rho_tolerance) {
+                        const double rho_new = rho_estimate(rho, prs, drs, fmax(nzs, naxs), fmax(npxs, natys));
+                        if (rho_changed(pm, rho_new, rho)) {
                             if (live) {
 #pragma unroll
                                 for (int k = 0; k < 11; ++k) {
@@ -1073,31 +1063,19 @@ struct Kk {
                     }
                 }
             }
-            if (status == PQP_UNSOLVED) {
-                const bool prim_ok = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
-                if (prim_ok && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
-                else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, 10 * pm.eps_prim_inf))
-                    status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
-                else status = PQP_MAX_ITER_REACHED;
-            }
+            if (status == PQP_UNSOLVED) status = max_iter_verdict(pm, res);
         }
         // ---- epilogue: getOptimizedPath (solver_k_as_input.cpp:22-44)
-        const bool has_sol = (status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED);
+        const bool has_sol = has_solution(status);
         c.sync();
         if (live) s.xr(2)[i] = x[2];
         c.sync();
         if (live) {
-            double ey = qnan, ephi = qnan, kk = qnan;
+            double ey = qnan, ephi = qnan, kk = qnan, tx, ty;
             if (has_sol) { ey = x[1]; ephi = x[0]; kk = last ? s.xr(2)[i - 1] : x[2]; }
-            const double angle = ref[i].z;
-            const double new_angle = constraint_angle(angle + 1.57079632679489661923);
-            const double tx = ref[i].x + ey * cos(new_angle), ty = ref[i].y + ey * sin(new_angle);
-            out[i].x = tx; out[i].y = ty; out[i].z = angle + ephi; out[i].k = kk; out[i].v = 0.0; out[i].a = 0.0;
+            optimized_station(ref[i], ey, ephi, kk, out[i], tx, ty);
             s.ox()[i] = tx; s.oy()[i] = ty;
-            if (bv.out_frenet) {
-                double *f = bv.out_frenet + 3 * (size_t)(off + i);
-                f[0] = ey; f[1] = ephi; f[2] = kk;
-            }
+            store_frenet(bv.out_frenet, off + i, ey, ephi, kk);
         }
         c.sync();
         if (tid == 0) {

@@ -814,8 +814,7 @@ PQP_DEV void kp_solve_path(Warp &w, const DevParams &prm, const BatchView &bv, i
         if (w.any(split)) status = PQP_INVALID_PROBLEM;
         else if (!kp_factor(w, cx)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
-        double pri_res = 0, dua_res = 0, pri_nrm = 0, dua_nrm = 0;
-        double inf_nrm = 0, inf_lhs = 0, inf_cert = 0;   // primal-infeasibility certificate of the last check
+        Residuals res{};   // of the last check
         // (without a workspace -- test harnesses of this core alone -- infeasibility is not detected)
         double *wold = bv.workspace ? kp_ws_wold(kp_ws_base(bv.workspace, off, prob), N) : nullptr;
         iter = 0;
@@ -1085,31 +1084,19 @@ PQP_DEV void kp_solve_path(Warp &w, const DevParams &prm, const BatchView &bv, i
                     }
 #undef PQP_G
 #undef PQP_ACC
-                    inf_nrm = w.max(c_nrm); inf_cert = w.max(c_cert); inf_lhs = w.sum(c_lhs);
+                    res.inf_nrm = w.max(c_nrm); res.inf_cert = w.max(c_cert); res.inf_lhs = w.sum(c_lhs);
                 }
                 pr = w.max(pr); nz = w.max(nz); nax = w.max(nax);
                 prs = w.max(prs); nzs = w.max(nzs); naxs = w.max(naxs);
                 dr = w.max(dr); npx = w.max(npx); naty = w.max(naty);
                 drs = w.max(drs); npxs = w.max(npxs); natys = w.max(natys);
                 w.sync();
-                pri_res = pr; dua_res = dr;
-                pri_nrm = fmax(nz, nax); dua_nrm = fmax(npx, naty);
-                if (can_check || iter == pm.max_iter) {
-                    // OSQP check_termination (unscaled residuals, strict <); ||q|| = 0, so the
-                    // dual-infeasibility test (q'dx < 0) never fires
-                    const bool prim_ok = pri_res < pm.eps_abs + pm.eps_rel * pri_nrm;
-                    if (pri_res > kOsqpInfty || dua_res > kOsqpInfty) status = PQP_NON_CVX;
-                    else if (prim_ok && dua_res < pm.eps_abs + pm.eps_rel * dua_nrm) status = PQP_SOLVED;
-                    else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, pm.eps_prim_inf))
-                        status = PQP_PRIMAL_INFEASIBLE;
-                }
+                res.pri_res = pr; res.dua_res = dr;
+                res.pri_nrm = fmax(nz, nax); res.dua_nrm = fmax(npx, naty);
+                if (can_check || iter == pm.max_iter) status = termination_verdict(pm, res);
                 if (status == PQP_UNSOLVED && can_adapt) {
-                    // OSQP compute_rho_estimate on the SCALED residuals
-                    const double pn = prs / (fmax(nzs, naxs) + 1e-10);
-                    const double dn = drs / (fmax(npxs, natys) + 1e-10);
-                    double rho_new = rho * sqrt(pn / (dn + 1e-10));
-                    rho_new = fmin(fmax(rho_new, kRhoMin), kRhoMax);
-                    if (rho_new > rho * pm.adaptive_rho_tolerance || rho_new < rho / pm.adaptive_rho_tolerance) {
+                    const double rho_new = rho_estimate(rho, prs, drs, fmax(nzs, naxs), fmax(npxs, natys));
+                    if (rho_changed(pm, rho_new, rho)) {
                         // y is kept, rho changes: w = E^-1 y / rho_row scales by rho/rho_new on every
                         // row whose rho follows the setting (free rows have w = 0).
                         const double ratio = rho / rho_new;
@@ -1141,36 +1128,21 @@ PQP_DEV void kp_solve_path(Warp &w, const DevParams &prm, const BatchView &bv, i
                 }
             }
         }
-        if (status == PQP_UNSOLVED) {
-            // max_iter reached: OSQP re-checks with 10x tolerances
-            const bool prim_ok = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
-            if (prim_ok && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
-            else if (!prim_ok && primal_infeasible(inf_nrm, inf_lhs, inf_cert, 10 * pm.eps_prim_inf))
-                status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
-            else status = PQP_MAX_ITER_REACHED;
-        }
+        if (status == PQP_UNSOLVED) status = max_iter_verdict(pm, res);
     }
     // ---- epilogue: getOptimizedPath, solver_kp_as_input.cpp:26-43
-    const bool has_sol = (status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED);
+    const bool has_sol = has_solution(status);
     const double nanv = nan("");
     for (int i = lane; i < N; i += 32) {
-        double ey = nanv, ephi = nanv, kk = nanv;
+        double ey = nanv, ephi = nanv, kk = nanv, tx, ty;
         if (has_sol) {
             const int ga = kp_gx(d, i);
             ey = s.xr()[ga]; ephi = s.xr()[ga + 1]; kk = s.xr()[ga + 2];
         }
-        const double angle = ref[i].z;
-        const double new_angle = constraint_angle(angle + 1.57079632679489661923);
-        const double tx = ref[i].x + ey * cos(new_angle);
-        const double ty = ref[i].y + ey * sin(new_angle);
-        out[i].x = tx; out[i].y = ty; out[i].z = angle + ephi; out[i].k = kk;
-        out[i].v = 0.0; out[i].a = 0.0;
+        optimized_station(ref[i], ey, ephi, kk, out[i], tx, ty);
         s.tr()[i] = tx;        // (tr/ts are free now)
         s.tmp()[i] = ty;
-        if (bv.out_frenet) {
-            double *f = bv.out_frenet + 3 * (size_t)(off + i);
-            f[0] = ey; f[1] = ephi; f[2] = kk;
-        }
+        store_frenet(bv.out_frenet, off + i, ey, ephi, kk);
     }
     w.sync();
     for (int i = lane; i < N; i += 32) {

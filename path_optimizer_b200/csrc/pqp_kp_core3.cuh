@@ -1866,29 +1866,14 @@ struct Kp3 {
 #undef PQP_CK
                     // No residual or certificate is carried across iterations (registers): the 10x
                     // re-check OSQP does when max_iter is reached is decided right here.
-                    const double pri_res = pr, dua_res = dr;
-                    const double pri_nrm = fmax(nz, nax), dua_nrm = fmax(npx, naty);
                     if (chk) {
-                        // OSQP check_termination; q = 0, so the dual-infeasibility test (q'dx < 0) never fires
-                        const bool prim_ok = pri_res < pm.eps_abs + pm.eps_rel * pri_nrm;
-                        if (pri_res > kOsqpInfty || dua_res > kOsqpInfty) status = PQP_NON_CVX;
-                        else if (prim_ok && dua_res < pm.eps_abs + pm.eps_rel * dua_nrm) status = PQP_SOLVED;
-                        else if (!prim_ok && primal_infeasible(c_nrm, c_lhs, c_cert, pm.eps_prim_inf))
-                            status = PQP_PRIMAL_INFEASIBLE;
-                        if (status == PQP_UNSOLVED && iter == pm.max_iter) {
-                            const bool prim_ok10 = pri_res < 10 * pm.eps_abs + 10 * pm.eps_rel * pri_nrm;
-                            if (prim_ok10 && dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * dua_nrm) status = PQP_SOLVED_INACCURATE;
-                            else if (!prim_ok10 && primal_infeasible(c_nrm, c_lhs, c_cert, 10 * pm.eps_prim_inf))
-                                status = PQP_PRIMAL_INFEASIBLE_INACCURATE;
-                            else status = PQP_MAX_ITER_REACHED;
-                        }
+                        const Residuals res{pr, dr, fmax(nz, nax), fmax(npx, naty), c_nrm, c_lhs, c_cert};
+                        status = termination_verdict(pm, res);
+                        if (status == PQP_UNSOLVED && iter == pm.max_iter) status = max_iter_verdict(pm, res);
                     }
                     if (status == PQP_UNSOLVED && can_adapt) {
-                        const double pn = prs / (fmax(nzs, naxs) + 1e-10);
-                        const double dn = drs / (fmax(npxs, natys) + 1e-10);
-                        double rho_new = rho * sqrt(pn / (dn + 1e-10));
-                        rho_new = fmin(fmax(rho_new, kRhoMin), kRhoMax);
-                        if (rho_new > rho * pm.adaptive_rho_tolerance || rho_new < rho / pm.adaptive_rho_tolerance) {
+                        const double rho_new = rho_estimate(rho, prs, drs, fmax(nzs, naxs), fmax(npxs, natys));
+                        if (rho_changed(pm, rho_new, rho)) {
                             const double ratio = rho / rho_new;   // y is kept: w = E^-1 y / rho_row rescales
                             double v, z;
 #define PQP_RESC(V, LO, HI) v = (V); z = clamp2(v, (LO), (HI)); (V) = z + (v - z) * ratio;
@@ -1995,24 +1980,16 @@ struct Kp3 {
         }
 #endif
         // ---- epilogue: getOptimizedPath, solver_kp_as_input.cpp:26-43
-        const bool has_sol = (status == PQP_SOLVED || status == PQP_SOLVED_INACCURATE || status == PQP_MAX_ITER_REACHED);
+        const bool has_sol = has_solution(status);
         c.sync();
         double *px = s.ex(0), *py = s.ex(1), *seg = s.ex(2);
         if (st.live) {
-            double ey = qnan, ephi = qnan, kk = qnan;
+            double ey = qnan, ephi = qnan, kk = qnan, tx, ty;
             if (has_sol) { ey = st.xa; ephi = st.xb; kk = st.xc; }
-            const double angle = ref[i].z;
-            const double new_angle = constraint_angle(angle + 1.57079632679489661923);
-            const double tx = ref[i].x + ey * cos(new_angle);
-            const double ty = ref[i].y + ey * sin(new_angle);
-            out[i].x = tx; out[i].y = ty; out[i].z = angle + ephi; out[i].k = kk;
-            out[i].v = 0.0; out[i].a = 0.0;
+            optimized_station(ref[i], ey, ephi, kk, out[i], tx, ty);
             px[i] = tx;
             py[i] = ty;
-            if (bv.out_frenet) {
-                double *f = bv.out_frenet + 3 * (size_t)(off + i);
-                f[0] = ey; f[1] = ephi; f[2] = kk;
-            }
+            store_frenet(bv.out_frenet, off + i, ey, ephi, kk);
         }
         c.sync();
         if (st.live) {
