@@ -217,6 +217,66 @@ int pqp_segment_reference_device(pqp_handle *h, int batch, const int32_t *d_knot
                                  int max_n_points, int capacity, int32_t *d_n_points, int32_t *d_offsets,
                                  pqp_state *d_ref, double *d_x0, double *d_end_heading, int32_t *d_ok, void *stream);
 
+/* Search a corridor around every smoothed reference line of a batch and post-smooth the line inside it, on DEVICE
+ * arrays of the handle's device: what ReferencePathSmoother::solve does after its smoother (graphSearchDp, then
+ * postSmooth), with outputs in the layout pqp_segment_reference_device takes.
+ *   d_knot_offsets, d_knots, d_x_coef, d_y_coef, d_max_s   every path's smoothed x(s), y(s) splines and length, the
+ *                      layout pqp_segment_reference_device takes
+ *   d_start            [batch] VehicleState's start state
+ *   d_map_index        [batch] every path's map in the handle's set, or NULL for map 0
+ *   search_lateral_range, search_lateral_spacing, search_longitudial_spacing   FLAGS_search_* (10, 0.6, 1.5)
+ *   max_layers         layers a path may have at most (>= 4)
+ *   capacity           knot rows the outputs hold
+ *   d_knot_offsets_out [batch+1] out: exclusive prefix of every path's knots (0 when refused); d_knot_offsets_out[batch]
+ *                      <= capacity (with batch = 0 the one entry 0 is written when the array is not NULL)
+ *   d_knots_out, d_x_coef_out [capacity][4], d_y_coef_out [capacity][4]   out: the post-smoothed lines' splines;
+ *                      rows past d_knot_offsets_out[batch] are not written
+ *   d_max_s_out        [batch] out: every line's new length, NaN when refused
+ *   d_ok               [batch] out: 1 when the path was post-smoothed, 0 when it was refused
+ *   d_status, d_iters  [batch] out: the post-smoothing QP's status and iterations; a path refused before its QP reports
+ *                      PQP_INVALID_PROBLEM and 0 iterations, as an empty problem does
+ *   d_layers           [capacity][3] out, or NULL: (layer s, lower bound, upper bound) of every kept layer, the
+ *                      reference's layers_s_list_ / layers_bounds_, in the knot rows of the path
+ * Per path, graphSearchDp (reference_path_smoother.cpp:145-301): the start's closest point on the line
+ * (findClosestPoint, tools.cpp:66-110: a 0.5 m grid scan and up to 20 Newton steps, clamped above by max_s only), the
+ * layers s += search_longitudial_spacing from it while below max_s, then max_s (0.5 m spacing for a line of 6 m or
+ * less); the start's lateral offset vehicle_l; a lattice of lateral nodes cur_l += spacing from -range while <= range
+ * per layer, a node feasible inside the map at distance >= 1.45 m and not past the turning radius on the inside, layer 0
+ * holding the start node alone; the DP of calculateCostAt (:110-143, weights 1, 0.5, 16 and 0.5, safe distance 3 m),
+ * its min over predecessors taken in index order with a strict '<'; the search stops at the first layer with no
+ * reachable node, backtracks from the cheapest node of the last layer reached, and marches each chosen node's bounds
+ * outwards in 0.2 m steps up to 6 m (layer 0: -10, 10).  Then postSmooth (:534-644): the QP with weights 1, 100 and
+ * 1000 on (offset, dx, ddx) of every layer, row 0 pinned to vehicle_l, solved with the handle's OSQP settings (the
+ * reference's OsqpEigen solvers set only verbosity and warm start, so under the default settings these are the
+ * settings postSmooth runs with); the points ref + offset * (cos, sin)(heading + pi/2), s accumulated, and the natural
+ * splines x(s), y(s) of tk::spline fitted through them.  The generic core's epilogue wraps heading + pi/2 into
+ * [-pi, pi] before its cosine and sine, so a point may differ from postSmooth's in the last bits.
+ * A path is refused (ok = 0, 0 knots, NaN max_s; no other path changes) when:
+ *   - its splines have fewer than 3 knots, or max_s <= 0, is not finite or exceeds 2^20 m (a grid scan too long);
+ *   - its start heading is not finite or exceeds 2^20 rad, or its closest point or vehicle_l is not finite;
+ *   - |vehicle_l| > search_lateral_range;
+ *   - it has more than max_layers layers, or the lateral lattice has more than 64 nodes;
+ *   - it reaches fewer than 4 layers;
+ *   - its QP does not end PQP_SOLVED, or its post-smoothed s is not strictly increasing;
+ *   - its map index lies outside the map set;
+ *   - the running total of knots, in index order, would pass capacity (as pqp_segment_reference_device's stations).
+ * NULL pointers (with batch > 0), a negative batch or capacity, max_layers < 4, flags that are not positive and finite,
+ * or no map set return PQP_ERR_ARG; a batch above the handle's max_batch, a capacity above its max_total_points or a
+ * max_layers whose QP does not fit one SM's shared memory (about 740 layers on an H100) PQP_ERR_CAPACITY; nothing is
+ * launched then.  Asynchronous on `stream` (NULL: the handle's stream), no host synchronisation; the scratch (about
+ * 0.6 KB per layer of max_layers per path of the handle's max_batch, and the kept points) is allocated by the first call
+ * and grows only with a larger max_layers, so after one call with the largest max_layers the call allocates nothing and
+ * can be captured in a CUDA graph ahead of pqp_segment_reference_device.
+ * Replaces: ReferencePathSmoother::graphSearchDp + ReferencePathSmoother::postSmooth (reference_path_smoother.cpp
+ * :145-301, :534-644), once per path. */
+int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offsets, const double *d_knots,
+                           const double *d_x_coef, const double *d_y_coef, const double *d_max_s,
+                           const pqp_state *d_start, const int32_t *d_map_index, double search_lateral_range,
+                           double search_lateral_spacing, double search_longitudial_spacing, int max_layers,
+                           int capacity, int32_t *d_knot_offsets_out, double *d_knots_out, double *d_x_coef_out,
+                           double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok, int32_t *d_status,
+                           int32_t *d_iters, double *d_layers, void *stream);
+
 /* tk::spline::operator() / deriv (spline.cpp:250-318) on a fitted spline; order 0..2. */
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at);
 

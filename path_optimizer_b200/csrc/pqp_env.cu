@@ -17,6 +17,9 @@
 #include "pqp_edt_core.cuh"
 #include "pqp_env_core.cuh"
 #include "pqp_segment_core.cuh"
+#include "pqp_corridor_core.cuh"
+#include "pqp_gen_core.cuh"
+#include "pqp_kernels.h"
 #include "pqp_dispatch.h"
 #include "pqp_handle.h"
 
@@ -60,6 +63,11 @@ struct EnvState {
     double *d_fit = nullptr;
     // pqp_segment_reference_device: every path's station count between its launches (max_batch, at first use)
     int32_t *d_seg = nullptr;
+    // pqp_post_smooth_device: the per-path search and QP state at a stride of cor_layers layers (max_batch paths), the
+    // kept paths' points (max_total) and per-path counters; grow-only, an outgrown blob is retired
+    char *d_cor = nullptr;
+    size_t cor_cap = 0;
+    int cor_layers = 0;
     // generic scratch for pqp_map_distance / pqp_check_states (grow-only)
     char *d_tmp = nullptr;
     size_t tmp_cap = 0;
@@ -71,7 +79,7 @@ void env_free(void *p) {
     cudaFree(e->d_map); cudaFree(e->d_maps); cudaFree(e->d_nmaps); cudaFree(e->d_mapidx); cudaFree(e->d_setidx);
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
-    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit); cudaFree(e->d_seg);
+    cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit); cudaFree(e->d_seg); cudaFree(e->d_cor);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     delete e;
 }
@@ -488,6 +496,241 @@ pqp_segment_write_kernel(const __grid_constant__ SegmentArgs a) {
     SplineView xs, ys;
     segment_splines(a, b, xs, ys);
     pqp::segment_write(a.f, xs, ys, a.n_points[b], a.ref + a.offsets[b]);
+}
+
+// pqp_post_smooth_device: six launches on the caller's stream.  (1) one warp per path runs graphSearchDp -- the grid
+// scan of findClosestPoint over its lanes, the DP with a lane per lateral node (two at most), the backtrack on lane 0,
+// the bound march with a lane per layer -- and assembles the post-smoothing QP in the generic core's band order;
+// (2) pqp_gen_solve_kernel solves it, its epilogue turning each layer's offset into the point
+// ref + offset * (cos, sin)(heading + pi/2) and accumulating s; (3) one thread per path keeps the path when the QP is
+// SOLVED and s strictly increasing; (4) the segment stage's one-warp reservation; (5) one thread per kept path copies
+// its points and layers to their reserved rows; (6) pqp_fit_splines_kernel fits x(s), y(s).  Between the launches
+// the per-path state sits in the handle's scratch, at a fixed stride of max_layers layers per path.
+struct CorridorArgs {
+    pqp::CorridorFlags f;
+    int batch, max_layers;
+    const int32_t *koff;
+    const double *knots, *xc, *yc, *max_s;
+    const pqp_state *start;
+    MapTable maps;
+    // scratch, per path: layers [Lm][3] (s, lower, upper), pred [Lm][64], feas [Lm], reason, and the QP in GenView form
+    double *layers;
+    int8_t *pred;
+    unsigned long long *feas;
+    int32_t *reason, *count;
+    int32_t *meta, *A_col, *Po_idx, *csc_ptr, *csc_row, *sep, *out_idx;
+    double *A_val, *l, *u, *Pd, *Po_val, *csc_val;
+    pqp_state *ref, *smooth, *compact;
+    const int32_t *status;
+    // outputs
+    const int32_t *offsets, *ok;
+    double *max_s_out, *layers_out;
+};
+
+__device__ __forceinline__ void corridor_refuse(const CorridorArgs &a, int b, int reason) {
+    if (threadIdx.x == 0) {
+        int32_t *mb = a.meta + (size_t)pqp::kGenMeta * b;
+        for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;   // n = 0: the generic core reports an empty problem
+        a.reason[b] = reason;
+    }
+}
+
+__global__ void __launch_bounds__(32)
+pqp_corridor_search_kernel(const __grid_constant__ CorridorArgs a) {
+    __shared__ double p_x[pqp::kCorridorMaxLateral], p_y[pqp::kCorridorMaxLateral], p_dir[pqp::kCorridorMaxLateral],
+        p_cost[pqp::kCorridorMaxLateral];
+    __shared__ unsigned char p_live[pqp::kCorridorMaxLateral];
+    const int b = blockIdx.x, lane = threadIdx.x;
+    const pqp::CorridorFlags &f = a.f;
+    const int Lm = a.max_layers;
+    const int o = a.koff[b], nk = a.koff[b + 1] - o;
+    const SplineView xs{nk, a.knots + o, a.xc + 4 * (size_t)o}, ys{nk, a.knots + o, a.yc + 4 * (size_t)o};
+    const double max_s = a.max_s[b];
+    const pqp_state start = a.start[b];
+    const MapView *mp = pqp::map_of(a.maps, b);
+    if (f.n_lat > pqp::kCorridorMaxLateral) return corridor_refuse(a, b, pqp::COR_WIDE);
+    if (!mp) return corridor_refuse(a, b, pqp::COR_MAP);
+    if (nk < 3) return corridor_refuse(a, b, pqp::COR_BAD_SPLINE);
+    if (!(max_s > 0.0 && max_s <= pqp::kCorridorMaxLength)) return corridor_refuse(a, b, pqp::COR_BAD_LENGTH);
+    if (!(fabs(start.z) <= pqp::kCorridorMaxHeading)) return corridor_refuse(a, b, pqp::COR_BAD_START);
+    const MapView m = *mp;
+    // findClosestPoint: the grid scan over the lanes, first index on a tie, then Newton on every lane alike
+    double best = pqp::kDblMax;
+    long long bk = 0;
+    const long long K = pqp::corridor_grid_count(max_s);
+    for (long long k = lane; k < K; k += 32) {
+        const double d = pqp::corridor_grid_dist(xs, ys, k, start.x, start.y);
+        if (d < best) { best = d; bk = k; }
+    }
+    for (int d = 16; d > 0; d >>= 1) {
+        const double ob = __shfl_xor_sync(0xffffffffu, best, d);
+        const long long ok_ = __shfl_xor_sync(0xffffffffu, bk, d);
+        if (ob < best || (ob == best && ok_ < bk)) { best = ob; bk = ok_; }
+    }
+    const double s0 = pqp::corridor_newton(xs, ys, start.x, start.y, 0.5 * (double)bk, max_s);
+    if (!isfinite(s0)) return corridor_refuse(a, b, pqp::COR_BAD_START);
+    // the layer lattice, accumulated on lane 0 (0.5 m spacing for a line of 6 m or less, :154)
+    double *lay = a.layers + (size_t)b * Lm * 3;
+    const double search_ds = max_s > 6 ? f.ds_long : 0.5;
+    int n_layers = 0;
+    if (lane == 0) {
+        double tmp = s0;
+        while (tmp < max_s && n_layers <= Lm) {
+            if (n_layers < Lm) lay[3 * n_layers] = tmp;
+            ++n_layers;
+            tmp = pqp::add(tmp, search_ds);
+        }
+        if (n_layers < Lm) lay[3 * n_layers] = max_s;
+        ++n_layers;
+    }
+    n_layers = __shfl_sync(0xffffffffu, n_layers, 0);
+    __syncwarp();
+    if (n_layers > Lm) return corridor_refuse(a, b, pqp::COR_TOO_MANY);
+    const double vl = pqp::corridor_vehicle_l(xs, ys, s0, start);
+    if (!isfinite(vl)) return corridor_refuse(a, b, pqp::COR_BAD_START);
+    if (fabs(vl) > f.range) return corridor_refuse(a, b, pqp::COR_FAR);
+    const int start_idx = (int)((f.range + vl) / f.spacing);
+    int8_t *pred = a.pred + (size_t)b * Lm * pqp::kCorridorMaxLateral;
+    unsigned long long *feas = a.feas + (size_t)b * Lm;
+    // layer 0: only the start node, feasible whatever the map says, with the start's heading and cost 0
+    {
+        const pqp_state r = pqp::densify_sample(xs, ys, s0);
+        const double an = r.z + M_PI_2, c_n = cos(an), s_n = sin(an);
+        for (int j = lane; j < f.n_lat; j += 32) {
+            p_x[j] = pqp::add(r.x, pqp::mul(f.lat[j], c_n));
+            p_y[j] = pqp::add(r.y, pqp::mul(f.lat[j], s_n));
+            p_live[j] = j == start_idx;
+            p_dir[j] = start.z;
+            p_cost[j] = j == start_idx ? 0.0 : pqp::kDblMax;
+        }
+        if (lane == 0) feas[0] = (start_idx >= 0 && start_idx < f.n_lat) ? 1ull << start_idx : 0ull;
+    }
+    __syncwarp();
+    int max_layer = 0;
+    for (int i = 1; i < n_layers; ++i) {
+        const double s = lay[3 * i], prev_s = lay[3 * (i - 1)];
+        const pqp_state r = pqp::densify_sample(xs, ys, s);
+        const double an = r.z + M_PI_2, c_n = cos(an), s_n = sin(an);
+        double nx[2], ny[2], nd[2], nc[2];
+        int np[2] = {-1, -1};
+        bool nf[2] = {false, false};
+        const pqp::CorridorPrev prev{p_x, p_y, p_dir, p_cost, p_live};
+        for (int h = 0; h < 2; ++h) {
+            const int j = lane + 32 * h;
+            if (j >= f.n_lat) continue;
+            const pqp::CorridorNode node = pqp::corridor_node(m, r, c_n, s_n, f.lat[j]);
+            nx[h] = node.x; ny[h] = node.y; nf[h] = node.feasible;
+            if (node.feasible) {
+                const double self = pqp::corridor_self_cost(node.dis, f.lat[j], f.range);
+                np[h] = pqp::corridor_relax(f, prev, prev_s, s, f.lat[j], r.z, node.x, node.y, self, &nc[h], &nd[h]);
+            }
+            pred[(size_t)i * pqp::kCorridorMaxLateral + j] = (int8_t)np[h];
+        }
+        const unsigned lo = __ballot_sync(0xffffffffu, nf[0]), hi = __ballot_sync(0xffffffffu, nf[1]);
+        const bool reached = __any_sync(0xffffffffu, np[0] >= 0 || np[1] >= 0);
+        if (lane == 0) feas[i] = (unsigned long long)lo | ((unsigned long long)hi << 32);
+        if (!reached) break;
+        __syncwarp();
+        for (int h = 0; h < 2; ++h) {
+            const int j = lane + 32 * h;
+            if (j >= f.n_lat) continue;
+            p_x[j] = nx[h]; p_y[j] = ny[h]; p_live[j] = np[h] >= 0;
+            p_dir[j] = np[h] >= 0 ? nd[h] : 0.0;
+            p_cost[j] = np[h] >= 0 ? nc[h] : pqp::kDblMax;
+        }
+        max_layer = i;
+        __syncwarp();
+    }
+    __syncwarp();
+    // the cheapest node of the last layer reached (strict '<'), and the backtrack with the rough bounds on lane 0
+    int R = 0;
+    if (lane == 0) {
+        double mc = pqp::kDblMax;
+        int j = -1;
+        for (int k = 0; k < f.n_lat; ++k)
+            if (p_cost[k] < mc) { mc = p_cost[k]; j = k; }
+        if (j >= 0) {
+            R = max_layer + 1;
+            for (int i = max_layer; i > 0; --i) {
+                pqp::corridor_rough(f, feas[i], j, &lay[3 * i + 1], &lay[3 * i + 2]);
+                j = pred[(size_t)i * pqp::kCorridorMaxLateral + j];
+            }
+        }
+    }
+    R = __shfl_sync(0xffffffffu, R, 0);
+    __syncwarp();
+    if (R < 4) return corridor_refuse(a, b, pqp::COR_SHORT);
+    // the bound march, a lane per layer, and the QP rows and columns each layer owns
+    pqp_state *ref = a.ref + (size_t)b * Lm;
+    const size_t on = (size_t)b * 3 * Lm, oz = (size_t)b * 7 * Lm, op = (size_t)b * (3 * Lm + 1);
+    for (int i = lane; i < R; i += 32) {
+        const pqp_state r = pqp::densify_sample(xs, ys, lay[3 * i]);
+        double lo = -10.0, hi = 10.0;
+        if (i > 0) pqp::corridor_march(m, r, lay[3 * i + 1], lay[3 * i + 2], &lo, &hi);
+        lay[3 * i + 1] = lo;
+        lay[3 * i + 2] = hi;
+        ref[i] = r;
+        const double ds = i + 1 < R ? lay[3 * (i + 1)] - lay[3 * i] : 0.0;
+        pqp::corridor_qp_rows(R, i, i == 0 ? vl : lo, i == 0 ? vl : hi, ds, a.A_col + 4 * on, a.A_val + 4 * on,
+                              a.l + on, a.u + on);
+        pqp::corridor_qp_columns(R, i, ds, a.csc_ptr + op, a.csc_row + oz, a.csc_val + oz);
+        for (int t = 0; t < 3; ++t) {
+            const size_t c = on + 3 * i + t;
+            a.Pd[c] = t == 0 ? 1.0 : t == 1 ? 100.0 : 1000.0;   // weight_x, weight_dx, weight_ddx (:595-597)
+            a.Po_idx[2 * c] = a.Po_idx[2 * c + 1] = -1;
+            a.Po_val[2 * c] = a.Po_val[2 * c + 1] = 0.0;
+            a.out_idx[3 * ((size_t)b * Lm + i) + t] = 3 * i + t;
+        }
+    }
+    if (lane == 0) {
+        int32_t *mb = a.meta + (size_t)pqp::kGenMeta * b;
+        const int M = pqp::corridor_qp_separators(R, a.sep + 32 * (size_t)b);
+        for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;
+        mb[0] = 3 * R; mb[1] = 3 * R - 2; mb[2] = 3 * R; mb[3] = 3; mb[4] = M; mb[5] = R;
+        mb[6] = (int32_t)((size_t)b * Lm); mb[7] = (int32_t)on; mb[8] = (int32_t)on; mb[9] = (int32_t)oz;
+        mb[10] = (int32_t)op;
+        a.reason[b] = pqp::COR_OK;
+    }
+}
+
+constexpr int kCorridorThreads = 128;
+
+// (3): a path keeps its R layers when its search succeeded, its QP is SOLVED and its s strictly increasing.
+__global__ void __launch_bounds__(kCorridorThreads)
+pqp_corridor_keep_kernel(const __grid_constant__ CorridorArgs a) {
+    const int b = blockIdx.x * kCorridorThreads + threadIdx.x;
+    if (b >= a.batch) return;
+    int reason = a.reason[b];
+    const int R = a.meta[(size_t)pqp::kGenMeta * b + 5];
+    if (reason == pqp::COR_OK && a.status[b] != PQP_SOLVED) reason = pqp::COR_QP;
+    if (reason == pqp::COR_OK) {
+        const pqp_state *p = a.smooth + (size_t)b * a.max_layers;
+        for (int i = 1; i < R; ++i)
+            if (!(p[i].s > p[i - 1].s)) reason = pqp::COR_S_ORDER;
+        if (!(p[R - 1].s <= pqp::kDblMax)) reason = pqp::COR_S_ORDER;
+    }
+    a.reason[b] = reason;
+    a.count[b] = reason == pqp::COR_OK ? R : 0;
+}
+
+// (5): a kept path's points and layers to its reserved rows, its length; NaN length for a refused one.
+__global__ void __launch_bounds__(kCorridorThreads)
+pqp_corridor_copy_kernel(const __grid_constant__ CorridorArgs a) {
+    const int b = blockIdx.x * kCorridorThreads + threadIdx.x;
+    if (b >= a.batch) return;
+    if (!a.ok[b]) {
+        a.max_s_out[b] = nan("");
+        return;
+    }
+    const int o = a.offsets[b], n = a.offsets[b + 1] - o;
+    const pqp_state *p = a.smooth + (size_t)b * a.max_layers;
+    const double *lay = a.layers + (size_t)b * a.max_layers * 3;
+    for (int i = 0; i < n; ++i) {
+        a.compact[o + i] = p[i];
+        if (a.layers_out)
+            for (int t = 0; t < 3; ++t) a.layers_out[3 * (size_t)(o + i) + t] = lay[3 * i + t];
+    }
+    a.max_s_out[b] = p[n - 1].s;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -977,6 +1220,129 @@ int pqp_segment_reference_device(pqp_handle *h, int batch, const int32_t *d_knot
     pqp_segment_scan_kernel<<<1, 32, 0, st>>>(a);
     PQP_CUDA(cudaGetLastError());
     pqp_segment_write_kernel<<<grid, kSegmentThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    return PQP_OK;
+}
+
+namespace {
+// The lateral lattice of graphSearchDp (:186-212): cur_l += spacing from -range while cur_l <= range.  Counts at most
+// kCorridorMaxLateral + 1 nodes; more than kCorridorMaxLateral refuses every path.
+void corridor_lattice(pqp::CorridorFlags *f) {
+    int n = 0;
+    for (double l = -f->range; l <= f->range && n <= pqp::kCorridorMaxLateral; l += f->spacing, ++n)
+        if (n < pqp::kCorridorMaxLateral) f->lat[n] = l;
+    f->n_lat = n;
+}
+
+// Carves the post-smoothing scratch for B paths of Lm layers and `total` kept points out of one blob.
+size_t corridor_carve(char *base, int B, int Lm, int total, CorridorArgs *a) {
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += (bytes + 255) & ~(size_t)255; return p; };
+    const size_t b = (size_t)B, L = (size_t)Lm;
+    a->layers = (double *)take(b * L * 3 * sizeof(double));
+    a->pred = (int8_t *)take(b * L * pqp::kCorridorMaxLateral);
+    a->feas = (unsigned long long *)take(b * L * sizeof(unsigned long long));
+    a->reason = (int32_t *)take(b * sizeof(int32_t));
+    a->count = (int32_t *)take(b * sizeof(int32_t));
+    a->meta = (int32_t *)take(b * pqp::kGenMeta * sizeof(int32_t));
+    a->A_col = (int32_t *)take(b * 3 * L * 4 * sizeof(int32_t));
+    a->A_val = (double *)take(b * 3 * L * 4 * sizeof(double));
+    a->l = (double *)take(b * 3 * L * sizeof(double));
+    a->u = (double *)take(b * 3 * L * sizeof(double));
+    a->Pd = (double *)take(b * 3 * L * sizeof(double));
+    a->Po_idx = (int32_t *)take(b * 3 * L * 2 * sizeof(int32_t));
+    a->Po_val = (double *)take(b * 3 * L * 2 * sizeof(double));
+    a->csc_ptr = (int32_t *)take(b * (3 * L + 1) * sizeof(int32_t));
+    a->csc_row = (int32_t *)take(b * 7 * L * sizeof(int32_t));
+    a->csc_val = (double *)take(b * 7 * L * sizeof(double));
+    a->sep = (int32_t *)take(b * 32 * sizeof(int32_t));
+    a->out_idx = (int32_t *)take(b * L * 3 * sizeof(int32_t));
+    a->ref = (pqp_state *)take(b * L * sizeof(pqp_state));
+    a->smooth = (pqp_state *)take(b * L * sizeof(pqp_state));
+    a->compact = (pqp_state *)take((size_t)total * sizeof(pqp_state));
+    return off;
+}
+}  // namespace
+
+int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offsets, const double *d_knots,
+                           const double *d_x_coef, const double *d_y_coef, const double *d_max_s,
+                           const pqp_state *d_start, const int32_t *d_map_index, double search_lateral_range,
+                           double search_lateral_spacing, double search_longitudial_spacing, int max_layers,
+                           int capacity, int32_t *d_knot_offsets_out, double *d_knots_out, double *d_x_coef_out,
+                           double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok, int32_t *d_status,
+                           int32_t *d_iters, double *d_layers, void *stream) {
+    auto flag_ok = [](double v) { return v > 0 && isfinite(v); };
+    if (!h || batch < 0 || capacity < 0 || max_layers < 4 || !flag_ok(search_lateral_range) ||
+        !flag_ok(search_lateral_spacing) || !flag_ok(search_longitudial_spacing) ||
+        (batch > 0 && (!d_knot_offsets || !d_knots || !d_x_coef || !d_y_coef || !d_max_s || !d_start ||
+                       !d_knot_offsets_out || !d_knots_out || !d_x_coef_out || !d_y_coef_out || !d_max_s_out || !d_ok ||
+                       !d_status || !d_iters))) {
+        pqp_set_err("pqp_post_smooth_device: bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (batch > h->max_batch || capacity > h->max_total) {
+        pqp_set_err("batch / capacity exceed what the handle was created for (max_batch, max_total_points)");
+        return PQP_ERR_CAPACITY;
+    }
+    if (max_layers > (1 << 20) ||
+        pqp::gen_smem_doubles(3 * max_layers, 3 * max_layers - 2, 3) * sizeof(double) > (size_t)h->smem_optin) {
+        pqp_set_err("pqp_post_smooth_device: max_layers too large for the post-smoothing QP of one path on one SM");
+        return PQP_ERR_CAPACITY;
+    }
+    EnvState *e;
+    int rc = need_map(h, &e);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    if (batch == 0) {                     // an empty batch still gets offsets[0] = 0 when the array is given
+        if (d_knot_offsets_out) PQP_CUDA(cudaMemsetAsync(d_knot_offsets_out, 0, sizeof(int32_t), st));
+        return PQP_OK;
+    }
+    CorridorArgs a{};
+    const int Lm = std::max(max_layers, e->cor_layers);
+    const size_t need = corridor_carve(nullptr, h->max_batch, Lm, h->max_total, &a) + 2 * (size_t)h->max_batch * 4;
+    if (need > e->cor_cap) {
+        if (e->d_cor) h->retired.push_back(e->d_cor);
+        e->d_cor = nullptr;
+        e->cor_cap = 0;
+        PQP_CUDA(cudaMalloc(&e->d_cor, need));
+        e->cor_cap = need;
+        e->cor_layers = Lm;
+    }
+    if (!e->d_fit) PQP_CUDA(cudaMalloc(&e->d_fit, (size_t)h->max_total * 4 * sizeof(double)));
+    const size_t carved = corridor_carve(e->d_cor, h->max_batch, max_layers, h->max_total, &a);
+    int32_t *n_points = (int32_t *)(e->d_cor + carved), *fit_ok = n_points + h->max_batch;
+    a.f.range = search_lateral_range; a.f.spacing = search_lateral_spacing; a.f.ds_long = search_longitudial_spacing;
+    corridor_lattice(&a.f);
+    a.batch = batch; a.max_layers = max_layers;
+    a.koff = d_knot_offsets; a.knots = d_knots; a.xc = d_x_coef; a.yc = d_y_coef; a.max_s = d_max_s; a.start = d_start;
+    a.maps = map_table(e, d_map_index);
+    a.status = d_status; a.offsets = d_knot_offsets_out; a.ok = d_ok; a.max_s_out = d_max_s_out; a.layers_out = d_layers;
+    pqp_corridor_search_kernel<<<batch, 32, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    pqp::GenView gv;
+    gv.batch = batch; gv.meta = a.meta; gv.A_col = a.A_col; gv.A_val = a.A_val; gv.l = a.l; gv.u = a.u; gv.Pd = a.Pd;
+    gv.Po_idx = a.Po_idx; gv.Po_val = a.Po_val; gv.csc_ptr = a.csc_ptr; gv.csc_row = a.csc_row; gv.csc_val = a.csc_val;
+    gv.sep = a.sep; gv.out_idx = a.out_idx; gv.ref = a.ref; gv.out_states = a.smooth; gv.out_frenet = nullptr;
+    gv.status = d_status; gv.iters = d_iters;
+    {
+        const size_t smem = pqp::gen_smem_doubles(3 * max_layers, 3 * max_layers - 2, 3) * sizeof(double);
+        int smem_doubles = (int)(smem / sizeof(double));
+        void *args[] = {(void *)&h->dprm, (void *)&gv, (void *)&smem_doubles};
+        PQP_CUDA(cudaLaunchKernel(pqp_gen_kernel_fn(), dim3(batch), dim3(32), args, smem, st));
+    }
+    const int grid = (batch + kCorridorThreads - 1) / kCorridorThreads;
+    pqp_corridor_keep_kernel<<<grid, kCorridorThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    SegmentArgs sa{};
+    sa.batch = batch; sa.capacity = capacity; sa.count = a.count;
+    sa.n_points = n_points; sa.offsets = d_knot_offsets_out; sa.ok = d_ok;
+    pqp_segment_scan_kernel<<<1, 32, 0, st>>>(sa);
+    PQP_CUDA(cudaGetLastError());
+    pqp_corridor_copy_kernel<<<grid, kCorridorThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    const FitArgs fa{batch, d_knot_offsets_out, a.compact, d_knots_out, d_x_coef_out, d_y_coef_out, e->d_fit, fit_ok};
+    pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(fa);
     PQP_CUDA(cudaGetLastError());
     return PQP_OK;
 }

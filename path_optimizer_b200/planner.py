@@ -342,6 +342,52 @@ class PathPlanner(BatchPathSolver):
             raise PqpError(f"pqp_segment_reference_device failed (rc={rc}): {_lib.last_error()}")
         return dict(n_points=n_points, offsets=offsets, ref=ref, x0=x0, end_heading=end_heading, ok=ok)
 
+    def post_smooth_device(self, splines, max_s, start, max_layers, capacity=None, map_index=None,
+                           search_lateral_range=10.0, search_lateral_spacing=0.6, search_longitudial_spacing=1.5,
+                           want_layers=False, out=None):
+        """ReferencePathSmoother's graphSearchDp + postSmooth for every path of a batch on the device
+        (pqp_post_smooth_device): smoothed lines in, post-smoothed lines out in the layout segment_device reads.
+        `splines` a dict of knot_offsets int32 [B + 1], knots [K], x_coef / y_coef [K, 4], max_s float64 [B] the lines'
+        lengths, start float64 [B, 7] the start states, map_index int32 [B] or None (map 0), all torch CUDA tensors; on
+        torch.cuda.current_stream().  The search flags default to the reference's.  max_layers: layers a path may have
+        at most; capacity: knot rows of the output (default the planner's max_total_points).  Returns
+        dict(knot_offsets int32 [B + 1], knots [capacity], x_coef / y_coef [capacity, 4], max_s [B], ok, status, iters
+        int32 [B], layers [capacity, 3] (s, lower, upper) with want_layers, else None).  A refused path gets ok = 0, 0
+        knots and NaN max_s.  No host synchronisation; after one call with the largest max_layers it can be captured in
+        a CUDA graph.  `out` may carry the output tensors, e.g. those of an earlier call."""
+        import torch
+        from . import device as D
+        dev = self._cuda_device()
+        B = int(max_s.shape[0])
+        cap = int(self.max_total_points if capacity is None else capacity)
+        K = int(splines["knots"].shape[0])
+        f64, i32 = torch.float64, torch.int32
+        out = dict(out or {})
+
+        def buf(name, shp, dtype):
+            return out[name] if out.get(name) is not None else torch.empty(shp, dtype=dtype, device=dev)
+        ko, kn = buf("knot_offsets", (B + 1,), i32), buf("knots", (cap,), f64)
+        xc, yc, ms = buf("x_coef", (cap, 4), f64), buf("y_coef", (cap, 4), f64), buf("max_s", (B,), f64)
+        ok, status, iters = buf("ok", (B,), i32), buf("status", (B,), i32), buf("iters", (B,), i32)
+        layers = buf("layers", (cap, 3), f64) if want_layers else None
+        rc = self._L.pqp_post_smooth_device(
+            self._h, B, D.check(splines["knot_offsets"], "knot_offsets", i32, (B + 1,), dev),
+            D.check(splines["knots"], "knots", f64, (K,), dev), D.check(splines["x_coef"], "x_coef", f64, (K, 4), dev),
+            D.check(splines["y_coef"], "y_coef", f64, (K, 4), dev), D.check(max_s, "max_s", f64, (B,), dev),
+            D.check(start, "start", f64, (B, D.STATE_COLS), dev),
+            None if map_index is None else D.check(map_index, "map_index", i32, (B,), dev),
+            float(search_lateral_range), float(search_lateral_spacing), float(search_longitudial_spacing),
+            int(max_layers), cap, D.check(ko, "knot_offsets", i32, (B + 1,), dev), D.check(kn, "knots", f64, (cap,), dev),
+            D.check(xc, "x_coef", f64, (cap, 4), dev), D.check(yc, "y_coef", f64, (cap, 4), dev),
+            D.check(ms, "max_s", f64, (B,), dev), D.check(ok, "ok", i32, (B,), dev),
+            D.check(status, "status", i32, (B,), dev), D.check(iters, "iters", i32, (B,), dev),
+            None if layers is None else D.check(layers, "layers", f64, (cap, 3), dev),
+            torch.cuda.current_stream(dev).cuda_stream)
+        if rc != OK:
+            raise PqpError(f"pqp_post_smooth_device failed (rc={rc}): {_lib.last_error()}")
+        return dict(knot_offsets=ko, knots=kn, x_coef=xc, y_coef=yc, max_s=ms, ok=ok, status=status, iters=iters,
+                    layers=layers)
+
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
                     collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None,
