@@ -277,6 +277,62 @@ int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offse
                            double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok, int32_t *d_status,
                            int32_t *d_iters, double *d_layers, void *stream);
 
+/* Smooth every raw reference polyline of a batch on DEVICE arrays of the handle's device: what
+ * ReferencePathSmoother::solve does before graphSearchDp under the default flags (smoothing_method TENSION2,
+ * tension_solver OSQP) -- the B-spline pre-pass, segmentRawReference and TensionSmoother2's smoothing QP -- with outputs
+ * in the layout pqp_post_smooth_device takes.
+ *   d_point_offsets    [batch+1] exclusive prefix of every path's input points
+ *   d_points           [d_point_offsets[batch]] the raw polylines; x and y are read
+ *   deviation_w, curvature_w, curvature_rate_w   FLAGS_tension_2_deviation_weight, _curvature_weight and
+ *                      _curvature_rate_weight (0.005, 1, 10)
+ *   max_raw_samples    B-spline samples a path may have at most (about its length in metres + 2)
+ *   max_points         resampled stations a path may have at most (ceil of its sampled length + 1)
+ *   capacity           knot rows the outputs hold
+ *   d_knot_offsets_out [batch+1] out: exclusive prefix of every path's knots (0 when refused); d_knot_offsets_out[batch]
+ *                      <= capacity (with batch = 0 the one entry 0 is written)
+ *   d_knots_out, d_x_coef_out [capacity][4], d_y_coef_out [capacity][4]   out: the smoothed lines' splines; rows past
+ *                      d_knot_offsets_out[batch] are not written
+ *   d_max_s_out        [batch] out: every smoothed line's length s.back() + 3, NaN when refused
+ *   d_ok               [batch] out: 1 when the path was smoothed, 0 when it was refused
+ *   d_status, d_iters  [batch] out: the smoothing QP's status and iterations; a path refused before its QP reports
+ *                      PQP_INVALID_PROBLEM and 0 iterations, as an empty problem does
+ * Per path: bSpline (reference_path_smoother.cpp:498-532) -- the length as the serial sum of distance() (tools.cpp:46),
+ * the degree 3, 4 or 5 from the average segment length (> 10, > 5, else), the clamped B-spline of that degree with the
+ * points as control points (tinyspline's BSpline(n, 2, degree), restated: clamped uniform knots and de Boor's
+ * algorithm), sampled at t += 1 / length (accumulated) while t < 1 and at t = 1, and s the serial sum of the sample
+ * distances; segmentRawReference (:50-88) -- the natural splines x(s), y(s) of tk::spline through the samples, sampled
+ * at s = 0, 1, 2, ... while s.back() < max_s (the last one extrapolated), with the heading atan2(dy, dx) and curvature
+ * (dx ddy - dy ddx) / pow(dx^2 + dy^2, 1.5); TensionSmoother2::osqpSmooth (tension_smoother_2.cpp:163-301) -- the QP in
+ * x, y, theta of every station and k of all but the last, with the three weights, the update rows and the pins of x_0,
+ * y_0, solved with the handle's OSQP settings (the reference's OsqpEigen solver sets only verbosity and warm start, so
+ * under the default settings these are the settings it runs with); and TensionSmoother::smooth's tail
+ * (tension_smoother.cpp:84-96) -- s accumulated from the solution's x, y, the natural splines x(s), y(s) fitted through
+ * them, max_s = s.back() + 3.  The IPOPT solver and the TENSION and ANGLE_DIFF methods are not restated.
+ * A path is refused (ok = 0, 0 knots, NaN max_s; no other path changes) when:
+ *   - it has fewer than 4 points (:36-39);
+ *   - the B-spline's degree is not below its point count (tinyspline refuses such a spline and the reference throws;
+ *     here it is a refusal), e.g. 4 or 5 points less than 5 m apart on average;
+ *   - its length is not positive and finite (a NaN or infinite coordinate);
+ *   - it has more than max_raw_samples B-spline samples, or more than max_points stations;
+ *   - its samples are fewer than 3 or their s is not strictly increasing, or it has fewer than 3 stations
+ *     (tk::spline::set_points asserts both, spline.cpp:164-165);
+ *   - its QP does not end PQP_SOLVED, or its smoothed s is not strictly increasing and finite;
+ *   - the running total of knots, in index order, would pass capacity (as pqp_segment_reference_device's stations).
+ * NULL pointers (with batch > 0), a negative batch or capacity, max_raw_samples or max_points below 3, or a weight that
+ * is negative or not finite return PQP_ERR_ARG; a batch above the handle's max_batch, a capacity above its
+ * max_total_points or a max_points whose QP does not fit one SM's shared memory (507 stations on an H100, 227 KB)
+ * PQP_ERR_CAPACITY; nothing is launched then.  Asynchronous on `stream` (NULL: the handle's stream), no host
+ * synchronisation; the scratch (about 0.2 KB per raw sample of max_raw_samples and 0.6 KB per station of max_points, per
+ * path of the handle's max_batch, and the kept points) is allocated by the first call and grows only with a larger
+ * max_raw_samples or max_points, so after one call with the largest caps the call allocates nothing and can be captured
+ * in a CUDA graph ahead of pqp_post_smooth_device.
+ * Replaces: ReferencePathSmoother::bSpline + TensionSmoother2::smooth (TENSION2, OSQP), once per path. */
+int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point_offsets, const pqp_state *d_points,
+                                double deviation_w, double curvature_w, double curvature_rate_w, int max_raw_samples,
+                                int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
+                                double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
+                                int32_t *d_status, int32_t *d_iters, void *stream);
+
 /* tk::spline::operator() / deriv (spline.cpp:250-318) on a fitted spline; order 0..2. */
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at);
 

@@ -18,6 +18,7 @@
 #include "pqp_env_core.cuh"
 #include "pqp_segment_core.cuh"
 #include "pqp_corridor_core.cuh"
+#include "pqp_smooth_core.cuh"
 #include "pqp_gen_core.cuh"
 #include "pqp_kernels.h"
 #include "pqp_dispatch.h"
@@ -68,6 +69,11 @@ struct EnvState {
     char *d_cor = nullptr;
     size_t cor_cap = 0;
     int cor_layers = 0;
+    // pqp_smooth_reference_device: the per-path samples, QP and solution at a stride of sm_raw samples and sm_points
+    // stations (max_batch paths), the kept paths' points (max_total) and per-path counters; grow-only, as d_cor
+    char *d_sm = nullptr;
+    size_t sm_cap = 0;
+    int sm_raw = 0, sm_points = 0;
     // generic scratch for pqp_map_distance / pqp_check_states (grow-only)
     char *d_tmp = nullptr;
     size_t tmp_cap = 0;
@@ -80,6 +86,7 @@ void env_free(void *p) {
     cudaFree(e->d_nvalid); cudaFree(e->d_nkept); cudaFree(e->d_ok); cudaFree(e->d_koff);
     cudaFree(e->d_spl); cudaFree(e->d_dense); cudaFree(e->d_knots); cudaFree(e->d_xc); cudaFree(e->d_yc);
     cudaFree(e->d_tmp); cudaFree(e->d_occ); cudaFree(e->d_edt); cudaFree(e->d_fit); cudaFree(e->d_seg); cudaFree(e->d_cor);
+    cudaFree(e->d_sm);
     for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
     delete e;
 }
@@ -733,6 +740,160 @@ pqp_corridor_copy_kernel(const __grid_constant__ CorridorArgs a) {
     a.max_s_out[b] = p[n - 1].s;
 }
 
+// pqp_smooth_reference_device: eight launches on the caller's stream.  (1) one warp per path checks the polyline, picks
+// the B-spline's degree, accumulates the sample parameters t on lane 0, evaluates de Boor's algorithm with a lane per
+// sample and sums s on lane 0; (2) pqp_fit_splines_kernel fits the raw x(s), y(s) -- over 2 batch "paths", path 2b
+// being path b's samples and path 2b + 1 the unused rest of its stride, which the fit refuses; (3) one warp per path
+// resamples at s = 0, 1, 2, ... with a lane per station and assembles the TENSION2 QP in band order; (4)
+// pqp_gen4_solve_kernel solves it, its epilogue copying (x_i, y_i, theta_i) to out_frenet; (5) one thread per path
+// accumulates s and keeps the path when its QP is SOLVED and s strictly increasing; (6) the segment stage's one-warp
+// reservation; (7) one thread per kept path copies its points to their reserved rows; (8) pqp_fit_splines_kernel fits
+// x(s), y(s).  Between the launches the per-path state sits in the handle's scratch, at fixed strides.
+struct SmoothArgs {
+    pqp::SmoothWeights w;
+    int batch, max_raw, max_points;
+    const int32_t *point_offsets;
+    const pqp_state *points;
+    // scratch
+    pqp_state *raw;                  // [B][max_raw] B-spline samples (x, y, s)
+    int32_t *raw_off, *raw_ok;       // [2B + 1], [2B]: the raw fit's "paths"
+    double *raw_knots, *raw_xc, *raw_yc, *raw_scr;
+    int32_t *reason, *count;
+    int32_t *meta, *A_col, *Po_idx, *csc_ptr, *csc_row, *sep, *out_idx;
+    double *A_val, *l, *u, *Pd, *Po_val, *q, *csc_val, *frenet;
+    pqp_state *ref, *smooth, *compact;
+    const int32_t *status;
+    // outputs
+    const int32_t *offsets, *ok;
+    double *max_s_out;
+};
+
+__device__ __forceinline__ void smooth_refuse(const SmoothArgs &a, int b, int reason) {
+    if (threadIdx.x == 0) {
+        int32_t *mb = a.meta + (size_t)pqp::kGenMeta * b;
+        for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;   // n = 0: the generic core reports an empty problem
+        a.reason[b] = reason;
+    }
+}
+
+__global__ void __launch_bounds__(32)
+pqp_smooth_sample_kernel(const __grid_constant__ SmoothArgs a) {
+    const int b = blockIdx.x, lane = threadIdx.x, Km = a.max_raw;
+    const int o = a.point_offsets[b], n = a.point_offsets[b + 1] - o;
+    pqp_state *raw = a.raw + (size_t)b * Km;
+    double *t = a.raw_knots + (size_t)b * Km;      // the parameters, until the raw fit copies s over them
+    int reason = pqp::SM_OK, K = 0;
+    if (n < 4) reason = pqp::SM_FEW;
+    const double *px = &a.points[o].x, *py = &a.points[o].y;
+    double length = 0;
+    int deg = 3;
+    if (reason == pqp::SM_OK) {
+        deg = pqp::smooth_degree(n, px, py, 7, &length);
+        if (deg >= n) reason = pqp::SM_DEGREE;
+        else if (!(length > 0 && length <= 1.7976931348623157e308)) reason = pqp::SM_LENGTH;
+    }
+    if (reason == pqp::SM_OK) {
+        if (lane == 0) K = pqp::smooth_sample_params(length, Km, t);
+        K = __shfl_sync(0xffffffffu, K, 0);
+        if (K > Km) reason = pqp::SM_RAW_MANY;
+    }
+    if (reason != pqp::SM_OK) K = 0;
+    __syncwarp();
+    for (int k = lane; k < K; k += 32) {
+        pqp_state &r = raw[k];
+        pqp::smooth_bspline_eval(n, deg, px, py, 7, t[k], &r.x, &r.y);
+        r.z = r.k = r.v = r.a = 0.0;
+    }
+    __syncwarp();
+    if (lane == 0) {
+        double s = 0;
+        for (int k = 0; k < K; ++k) {
+            if (k > 0) s = pqp::add(s, pqp::smooth_step(raw[k - 1].x, raw[k - 1].y, raw[k].x, raw[k].y));
+            raw[k].s = s;
+        }
+        if (K < Km) raw[K].s = nan("");           // the rest of the stride: a path the raw fit refuses
+        a.raw_off[2 * b] = b * Km;
+        a.raw_off[2 * b + 1] = b * Km + K;
+        if (b + 1 == a.batch) a.raw_off[2 * a.batch] = a.batch * Km;
+        if (reason != pqp::SM_OK) smooth_refuse(a, b, reason);
+        else a.reason[b] = pqp::SM_OK;
+    }
+}
+
+__global__ void __launch_bounds__(32)
+pqp_smooth_assemble_kernel(const __grid_constant__ SmoothArgs a) {
+    const int b = blockIdx.x, lane = threadIdx.x, Km = a.max_raw, Nm = a.max_points;
+    if (a.reason[b] != pqp::SM_OK) return;
+    if (!a.raw_ok[2 * b]) return smooth_refuse(a, b, pqp::SM_RAW_ORDER);
+    const int K = a.raw_off[2 * b + 1] - a.raw_off[2 * b];
+    const size_t ro = (size_t)b * Km;
+    const SplineView xs{K, a.raw_knots + ro, a.raw_xc + 4 * ro}, ys{K, a.raw_knots + ro, a.raw_yc + 4 * ro};
+    const double max_s = a.raw_knots[ro + K - 1];
+    if (!(max_s <= (double)Nm)) return smooth_refuse(a, b, pqp::SM_MANY);
+    const int N = pqp::smooth_station_count(max_s);
+    if (N > Nm) return smooth_refuse(a, b, pqp::SM_MANY);
+    if (N < 3) return smooth_refuse(a, b, pqp::SM_SHORT);
+    const double x0 = pqp::spline_eval(xs, 0, 0.0), y0 = pqp::spline_eval(ys, 0, 0.0);
+    const size_t oN = (size_t)b * Nm, on = 4 * oN, om = 3 * oN, oz = 9 * oN, op = (size_t)b * (4 * Nm + 1);
+    for (int i = lane; i < N; i += 32) {
+        const pqp_state st = pqp::densify_sample(xs, ys, (double)i);
+        a.ref[oN + i] = st;
+        pqp::smooth_qp_station(N, i, st, (double)(i + 1) - (double)i, x0, y0, a.w, a.A_col + 4 * om, a.A_val + 4 * om,
+                               a.l + om, a.u + om, a.Pd + on, a.Po_idx + 2 * on, a.Po_val + 2 * on, a.q + on,
+                               a.csc_ptr + op, a.csc_row + oz, a.csc_val + oz);
+        for (int t = 0; t < 3; ++t) a.out_idx[3 * (oN + i) + t] = 4 * i + t;
+    }
+    if (lane == 0) {
+        int32_t *mb = a.meta + (size_t)pqp::kGenMeta * b;
+        const int M = pqp::smooth_qp_separators(N, a.sep + 32 * (size_t)b);
+        for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;
+        mb[0] = 4 * N - 1; mb[1] = 3 * N - 1; mb[2] = 4 * N - 1; mb[3] = 4; mb[4] = M; mb[5] = N;
+        mb[6] = (int32_t)oN; mb[7] = (int32_t)on; mb[8] = (int32_t)om; mb[9] = (int32_t)oz; mb[10] = (int32_t)op;
+    }
+}
+
+constexpr int kSmoothThreads = 128;
+
+// (5): s accumulated from the solution's (x, y) (osqpSmooth's output loop); a path keeps its N stations when its QP is
+// SOLVED and its s strictly increasing and finite.
+__global__ void __launch_bounds__(kSmoothThreads)
+pqp_smooth_keep_kernel(const __grid_constant__ SmoothArgs a) {
+    const int b = blockIdx.x * kSmoothThreads + threadIdx.x;
+    if (b >= a.batch) return;
+    int reason = a.reason[b];
+    const int N = a.meta[(size_t)pqp::kGenMeta * b + 5];
+    if (reason == pqp::SM_OK && a.status[b] != PQP_SOLVED) reason = pqp::SM_QP;
+    if (reason == pqp::SM_OK) {
+        const double *f = a.frenet + 3 * (size_t)b * a.max_points;
+        pqp_state *p = a.smooth + (size_t)b * a.max_points;
+        double s = 0;
+        for (int i = 0; i < N; ++i) {
+            const double x = f[3 * i], y = f[3 * i + 1];
+            if (i > 0) s = pqp::add(s, pqp::smooth_step(p[i - 1].x, p[i - 1].y, x, y));
+            if (i > 0 && !(s > p[i - 1].s)) reason = pqp::SM_S_ORDER;
+            p[i].x = x; p[i].y = y; p[i].s = s;
+        }
+        if (!(s <= 1.7976931348623157e308)) reason = pqp::SM_S_ORDER;
+    }
+    a.reason[b] = reason;
+    a.count[b] = reason == pqp::SM_OK ? N : 0;
+}
+
+// (7): a kept path's points to its reserved rows and its length s.back() + 3; NaN length for a refused one.
+__global__ void __launch_bounds__(kSmoothThreads)
+pqp_smooth_copy_kernel(const __grid_constant__ SmoothArgs a) {
+    const int b = blockIdx.x * kSmoothThreads + threadIdx.x;
+    if (b >= a.batch) return;
+    if (!a.ok[b]) {
+        a.max_s_out[b] = nan("");
+        return;
+    }
+    const int o = a.offsets[b], n = a.offsets[b + 1] - o;
+    const pqp_state *p = a.smooth + (size_t)b * a.max_points;
+    for (int i = 0; i < n; ++i) a.compact[o + i] = p[i];
+    a.max_s_out[b] = pqp::add(p[n - 1].s, 3.0);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host helpers
 // ---------------------------------------------------------------------------------------------
@@ -1340,6 +1501,131 @@ int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offse
     pqp_segment_scan_kernel<<<1, 32, 0, st>>>(sa);
     PQP_CUDA(cudaGetLastError());
     pqp_corridor_copy_kernel<<<grid, kCorridorThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    const FitArgs fa{batch, d_knot_offsets_out, a.compact, d_knots_out, d_x_coef_out, d_y_coef_out, e->d_fit, fit_ok};
+    pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(fa);
+    PQP_CUDA(cudaGetLastError());
+    return PQP_OK;
+}
+
+namespace {
+// Carves the smoothing scratch for B paths of Km raw samples and Nm stations and `total` kept points out of one blob.
+size_t smooth_carve(char *base, int B, int Km, int Nm, int total, SmoothArgs *a) {
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += (bytes + 255) & ~(size_t)255; return p; };
+    const size_t b = (size_t)B, K = (size_t)Km, N = (size_t)Nm;
+    a->raw = (pqp_state *)take(b * K * sizeof(pqp_state));
+    a->raw_off = (int32_t *)take((2 * b + 1) * sizeof(int32_t));
+    a->raw_ok = (int32_t *)take(2 * b * sizeof(int32_t));
+    a->raw_knots = (double *)take(b * K * sizeof(double));
+    a->raw_xc = (double *)take(b * K * 4 * sizeof(double));
+    a->raw_yc = (double *)take(b * K * 4 * sizeof(double));
+    a->raw_scr = (double *)take(b * K * 4 * sizeof(double));
+    a->reason = (int32_t *)take(b * sizeof(int32_t));
+    a->count = (int32_t *)take(b * sizeof(int32_t));
+    a->meta = (int32_t *)take(b * pqp::kGenMeta * sizeof(int32_t));
+    a->A_col = (int32_t *)take(b * 3 * N * 4 * sizeof(int32_t));
+    a->A_val = (double *)take(b * 3 * N * 4 * sizeof(double));
+    a->l = (double *)take(b * 3 * N * sizeof(double));
+    a->u = (double *)take(b * 3 * N * sizeof(double));
+    a->Pd = (double *)take(b * 4 * N * sizeof(double));
+    a->q = (double *)take(b * 4 * N * sizeof(double));
+    a->Po_idx = (int32_t *)take(b * 4 * N * 2 * sizeof(int32_t));
+    a->Po_val = (double *)take(b * 4 * N * 2 * sizeof(double));
+    a->csc_ptr = (int32_t *)take(b * (4 * N + 1) * sizeof(int32_t));
+    a->csc_row = (int32_t *)take(b * 9 * N * sizeof(int32_t));
+    a->csc_val = (double *)take(b * 9 * N * sizeof(double));
+    a->sep = (int32_t *)take(b * 32 * sizeof(int32_t));
+    a->out_idx = (int32_t *)take(b * N * 3 * sizeof(int32_t));
+    a->frenet = (double *)take(b * N * 3 * sizeof(double));
+    a->ref = (pqp_state *)take(b * N * sizeof(pqp_state));
+    a->smooth = (pqp_state *)take(b * N * sizeof(pqp_state));
+    a->compact = (pqp_state *)take((size_t)total * sizeof(pqp_state));
+    return off;
+}
+}  // namespace
+
+int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point_offsets, const pqp_state *d_points,
+                                double deviation_w, double curvature_w, double curvature_rate_w, int max_raw_samples,
+                                int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
+                                double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
+                                int32_t *d_status, int32_t *d_iters, void *stream) {
+    auto weight_ok = [](double v) { return v >= 0 && isfinite(v); };
+    if (!h || batch < 0 || capacity < 0 || max_raw_samples < 3 || max_points < 3 || !weight_ok(deviation_w) ||
+        !weight_ok(curvature_w) || !weight_ok(curvature_rate_w) ||
+        (batch > 0 && (!d_point_offsets || !d_points || !d_knot_offsets_out || !d_knots_out || !d_x_coef_out ||
+                       !d_y_coef_out || !d_max_s_out || !d_ok || !d_status || !d_iters))) {
+        pqp_set_err("pqp_smooth_reference_device: bad argument");
+        return PQP_ERR_ARG;
+    }
+    if (batch > h->max_batch || capacity > h->max_total) {
+        pqp_set_err("batch / capacity exceed what the handle was created for (max_batch, max_total_points)");
+        return PQP_ERR_CAPACITY;
+    }
+    if (max_points > (1 << 20) ||
+        pqp::gen_smem_doubles<4>(4 * max_points - 1, 3 * max_points - 1, 4) * sizeof(double) > (size_t)h->smem_optin ||
+        (size_t)h->max_batch * 9 * max_points > (size_t)INT32_MAX ||
+        (size_t)h->max_batch * max_raw_samples > (size_t)INT32_MAX) {
+        pqp_set_err("pqp_smooth_reference_device: max_points too large for the smoothing QP of one path on one SM, or "
+                    "max_batch x max_raw_samples / max_points beyond 32-bit offsets");
+        return PQP_ERR_CAPACITY;
+    }
+    EnvState *e;
+    int rc = env_get(h, &e);
+    if (rc != PQP_OK) return rc;
+    PQP_CUDA(cudaSetDevice(h->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    if (batch == 0) {                     // an empty batch still gets offsets[0] = 0 when the array is given
+        if (d_knot_offsets_out) PQP_CUDA(cudaMemsetAsync(d_knot_offsets_out, 0, sizeof(int32_t), st));
+        return PQP_OK;
+    }
+    SmoothArgs a{};
+    const int Km = std::max(max_raw_samples, e->sm_raw), Nm = std::max(max_points, e->sm_points);
+    const size_t need = smooth_carve(nullptr, h->max_batch, Km, Nm, h->max_total, &a) + 2 * (size_t)h->max_batch * 4;
+    if (need > e->sm_cap) {
+        if (e->d_sm) h->retired.push_back(e->d_sm);
+        e->d_sm = nullptr;
+        e->sm_cap = 0;
+        PQP_CUDA(cudaMalloc(&e->d_sm, need));
+        e->sm_cap = need;
+        e->sm_raw = Km;
+        e->sm_points = Nm;
+    }
+    if (!e->d_fit) PQP_CUDA(cudaMalloc(&e->d_fit, (size_t)h->max_total * 4 * sizeof(double)));
+    const size_t carved = smooth_carve(e->d_sm, h->max_batch, max_raw_samples, max_points, h->max_total, &a);
+    int32_t *n_points = (int32_t *)(e->d_sm + carved), *fit_ok = n_points + h->max_batch;
+    a.w = pqp::SmoothWeights{deviation_w, curvature_w, curvature_rate_w};
+    a.batch = batch; a.max_raw = max_raw_samples; a.max_points = max_points;
+    a.point_offsets = d_point_offsets; a.points = d_points;
+    a.status = d_status; a.offsets = d_knot_offsets_out; a.ok = d_ok; a.max_s_out = d_max_s_out;
+    pqp_smooth_sample_kernel<<<batch, 32, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    const FitArgs ra{2 * batch, a.raw_off, a.raw, a.raw_knots, a.raw_xc, a.raw_yc, a.raw_scr, a.raw_ok};
+    pqp_fit_splines_kernel<<<(2 * batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(ra);
+    PQP_CUDA(cudaGetLastError());
+    pqp_smooth_assemble_kernel<<<batch, 32, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    pqp::GenView gv;
+    gv.batch = batch; gv.meta = a.meta; gv.A_col = a.A_col; gv.A_val = a.A_val; gv.l = a.l; gv.u = a.u; gv.Pd = a.Pd;
+    gv.Po_idx = a.Po_idx; gv.Po_val = a.Po_val; gv.csc_ptr = a.csc_ptr; gv.csc_row = a.csc_row; gv.csc_val = a.csc_val;
+    gv.sep = a.sep; gv.out_idx = a.out_idx; gv.ref = a.ref; gv.out_states = a.smooth; gv.out_frenet = a.frenet;
+    gv.status = d_status; gv.iters = d_iters;
+    {
+        const size_t smem = pqp::gen_smem_doubles<4>(4 * max_points - 1, 3 * max_points - 1, 4) * sizeof(double);
+        int smem_doubles = (int)(smem / sizeof(double));
+        const double *q = a.q;
+        void *args[] = {(void *)&h->dprm, (void *)&gv, (void *)&smem_doubles, (void *)&q};
+        PQP_CUDA(cudaLaunchKernel(pqp_gen4_kernel_fn(), dim3(batch), dim3(32), args, smem, st));
+    }
+    const int grid = (batch + kSmoothThreads - 1) / kSmoothThreads;
+    pqp_smooth_keep_kernel<<<grid, kSmoothThreads, 0, st>>>(a);
+    PQP_CUDA(cudaGetLastError());
+    SegmentArgs sa{};
+    sa.batch = batch; sa.capacity = capacity; sa.count = a.count;
+    sa.n_points = n_points; sa.offsets = d_knot_offsets_out; sa.ok = d_ok;
+    pqp_segment_scan_kernel<<<1, 32, 0, st>>>(sa);
+    PQP_CUDA(cudaGetLastError());
+    pqp_smooth_copy_kernel<<<grid, kSmoothThreads, 0, st>>>(a);
     PQP_CUDA(cudaGetLastError());
     const FitArgs fa{batch, d_knot_offsets_out, a.compact, d_knots_out, d_x_coef_out, d_y_coef_out, e->d_fit, fit_ok};
     pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(fa);

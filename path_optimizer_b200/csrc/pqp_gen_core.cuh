@@ -4,8 +4,10 @@
 //   "KPC" SolverKpAsInputConstrained   reference src/solver/solver_kp_as_input_constrained.cpp:13-221
 // The host (pqp_forms.h) restates the reference's setHessianMatrix / setConstraintMatrix as sparse
 // rows (<= 4 entries per row, as every row of these formulations has), orders the unknowns station
-// by station so that the reduced KKT  cP + sigma D^-2 + A' W A  is banded, and marks 3-unknown
-// separators (one station's state) every L stations.  The device part is formulation-agnostic:
+// by station so that the reduced KKT  cP + sigma D^-2 + A' W A  is banded, and marks S-unknown
+// separators (one station's unknowns) every L stations: S = 3 for "K" and "KPC", S = 4 for the TENSION2
+// smoothing QP of pqp_smooth_reference_device, whose four chains x, y, theta, k admit no 3-unknown separator.
+// That QP also has a linear cost term q (kLinear); the formulations above have q = 0.  The device part is formulation-agnostic:
 // OSQP's Ruiz scaling / rho classes / ADMM recurrence / termination / adaptive rho exactly as in
 // pqp_kp_core.cuh (same unscaled-weighted form, same partitioned banded LDL'), with the stencils
 // replaced by ELL row gathers and CSC column gathers.
@@ -39,8 +41,47 @@ struct GenView {
     int32_t *status, *iters; // [B]
 };
 
+// Per-lane reduction record of an S-wide separator: [0, S^2) Dg / Sinv, [S^2, 2S^2) Off, [2S^2, 3S^2) G,
+// [3S^2, 4S^2) A, [4S^2, 5S^2) C, [5S^2, 5S^2 + S) g.  S = 3 gives kRedStride.
+template <int S> constexpr int kGenRedStride = 5 * S * S + S;
+static_assert(kGenRedStride<3> == kRedStride, "width-3 record");
+
+template <int S = 3>
 PQP_HD size_t gen_smem_doubles(int n, int m, int bw) {
-    return 5 * (size_t)n + 4 * (size_t)m + (size_t)(bw + 1) * n + (size_t)kRedStride * 32;
+    return 5 * (size_t)n + 4 * (size_t)m + (size_t)(bw + 1) * n + (size_t)kGenRedStride<S> * 32;
+}
+
+// Inverse of an SPD S x S block (row-major), S = 3 through inv3_spd, S = 4 by LDL'.
+template <int S> PQP_DEV void gen_inv_spd(const double *a, double *o) {
+    if constexpr (S == 3) {
+        inv3_spd(a, o);
+    } else {
+        double L[S * S], d[S];
+        for (int j = 0; j < S; ++j) {
+            double dj = a[j * S + j];
+            for (int k = 0; k < j; ++k) dj -= L[j * S + k] * L[j * S + k] * d[k];
+            d[j] = dj;
+            for (int i = j + 1; i < S; ++i) {
+                double v = a[i * S + j];
+                for (int k = 0; k < j; ++k) v -= L[i * S + k] * L[j * S + k] * d[k];
+                L[i * S + j] = v / dj;
+            }
+        }
+        // inv = L^-T diag(1/d) L^-1, column c of L^-1 by forward substitution
+        double Mi[S * S];
+        for (int c = 0; c < S; ++c)
+            for (int i = 0; i < S; ++i) {
+                double v = i == c ? 1.0 : 0.0;
+                for (int k = c; k < i; ++k) v -= L[i * S + k] * Mi[k * S + c];
+                Mi[i * S + c] = v;
+            }
+        for (int r = 0; r < S; ++r)
+            for (int c = r; c < S; ++c) {
+                double v = 0.0;
+                for (int k = c; k < S; ++k) v += Mi[k * S + r] * Mi[k * S + c] / d[k];
+                o[r * S + c] = o[c * S + r] = v;
+            }
+    }
 }
 
 struct GenCtx {
@@ -52,6 +93,17 @@ struct GenCtx {
 };
 
 #define PQP_GB(g, dd) cx.band[(size_t)(g) * (cx.bw + 1) + (dd)]
+
+// a[0] b[0] + a[1] b[1] + ... in that order (S = 3: the expression the width-3 core always had)
+template <int S> PQP_DEV double gen_dot(const double *a, const double *b) {
+    if constexpr (S == 3) {
+        return a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
+    } else {
+        double acc = a[0] * b[0];
+        for (int k = 1; k < S; ++k) acc += a[k] * b[k];
+        return acc;
+    }
+}
 
 PQP_DEV int gen_local_factor(const GenCtx &cx, int lo, int hi) {
     const int bw = cx.bw;
@@ -90,7 +142,9 @@ PQP_DEV void gen_local_solve(const GenCtx &cx, double *v, int lo, int hi) {
 }
 
 // band assembly (one thread per band row, deterministic) + partitioned factorisation
+template <int S>
 PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
+    constexpr int RS = kGenRedStride<S>, S2 = S * S;
     const int n = cx.n, bw = cx.bw, lane = w.lane();
     for (int j = lane; j < n; j += 32) {
         for (int dd = 0; dd <= bw; ++dd) PQP_GB(j, dd) = 0.0;
@@ -113,18 +167,18 @@ PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
     w.sync();
     int ok = 1;
     const bool act = lane < cx.M;
-    double *R = cx.red + (size_t)kRedStride * lane;
+    double *R = cx.red + (size_t)RS * lane;
     if (act) ok = gen_local_factor(cx, cx.lo, cx.hi);
     w.sync();
     if (act) {
         const int lo = cx.lo, hi = cx.hi, gs = cx.gsep, gq = hi;
         const bool has_right = (lane + 1 < cx.M);
-        for (int k = 9; k < 18; ++k) R[k] = 0.0;
-        for (int k = 27; k < 45; ++k) R[k] = 0.0;
-        for (int col = 0; col < 6; ++col) {
-            const bool left = col < 3;
+        for (int k = S2; k < 2 * S2; ++k) R[k] = 0.0;
+        for (int k = 3 * S2; k < 5 * S2; ++k) R[k] = 0.0;
+        for (int col = 0; col < 2 * S; ++col) {
+            const bool left = col < S;
             if (!left && !has_right) break;
-            const int sc = left ? gs + col : gq + (col - 3);
+            const int sc = left ? gs + col : gq + (col - S);
             for (int g = lo; g < hi; ++g) {
                 double vv = 0.0;
                 if (left) { if (g - sc <= bw) vv = PQP_GB(g, g - sc); }
@@ -132,7 +186,7 @@ PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
                 cx.tmp[g] = vv;
             }
             gen_local_solve(cx, cx.tmp, lo, hi);
-            for (int r = 0; r < 3; ++r) {
+            for (int r = 0; r < S; ++r) {
                 double accL = 0.0, accR = 0.0;
                 const int sl = gs + r, sr = gq + r;
                 for (int g = lo; g < hi && g - sl <= bw; ++g) accL += PQP_GB(g, g - sl) * cx.tmp[g];
@@ -141,46 +195,46 @@ PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
                     if (g0 < lo) g0 = lo;
                     for (int g = g0; g < hi; ++g) accR += PQP_GB(sr, sr - g) * cx.tmp[g];
                 }
-                if (left) { R[27 + r * 3 + col] = accL; R[9 + col * 3 + r] = -accR; }
-                else R[36 + r * 3 + (col - 3)] = accR;
+                if (left) { R[3 * S2 + r * S + col] = accL; R[S2 + col * S + r] = -accR; }
+                else R[4 * S2 + r * S + (col - S)] = accR;
             }
         }
     }
     w.sync();
     if (act) {
         const int gs = cx.gsep;
-        const double *Cprev = cx.red + (size_t)kRedStride * (lane - 1) + 36;
-        for (int r = 0; r < 3; ++r)
-            for (int cc = 0; cc < 3; ++cc) {
+        const double *Cprev = cx.red + (size_t)RS * (lane - 1) + 4 * S2;
+        for (int r = 0; r < S; ++r)
+            for (int cc = 0; cc < S; ++cc) {
                 const int hi_ = r > cc ? r : cc, lo_ = r > cc ? cc : r;
-                double vv = PQP_GB(gs + hi_, hi_ - lo_) - R[27 + r * 3 + cc];
-                if (lane > 0) vv -= Cprev[r * 3 + cc];
-                R[r * 3 + cc] = vv;
+                double vv = PQP_GB(gs + hi_, hi_ - lo_) - R[3 * S2 + r * S + cc];
+                if (lane > 0) vv -= Cprev[r * S + cc];
+                R[r * S + cc] = vv;
             }
     }
     w.sync();
     if (lane == 0) {
-        double Sch[9], Sinv[9];
-        for (int k = 0; k < 9; ++k) Sch[k] = cx.red[k];
+        double Sch[S2], Sinv[S2];
+        for (int k = 0; k < S2; ++k) Sch[k] = cx.red[k];
         for (int p = 0; p < cx.M; ++p) {
-            double *Rp = cx.red + (size_t)kRedStride * p;
+            double *Rp = cx.red + (size_t)RS * p;
             if (!(Sch[0] > 0.0)) ok = 0;
-            inv3_spd(Sch, Sinv);
-            for (int k = 0; k < 9; ++k) Rp[k] = Sinv[k];
+            gen_inv_spd<S>(Sch, Sinv);
+            for (int k = 0; k < S2; ++k) Rp[k] = Sinv[k];
             if (p + 1 < cx.M) {
-                double *Rn = Rp + kRedStride;
-                const double *Off = Rp + 9;
-                for (int r = 0; r < 3; ++r)
-                    for (int cc = 0; cc < 3; ++cc) {
+                double *Rn = Rp + RS;
+                const double *Off = Rp + S2;
+                for (int r = 0; r < S; ++r)
+                    for (int cc = 0; cc < S; ++cc) {
                         double a = 0.0;
-                        for (int k = 0; k < 3; ++k) a += Off[k * 3 + r] * Sinv[k * 3 + cc];
-                        Rn[18 + r * 3 + cc] = a;
+                        for (int k = 0; k < S; ++k) a += Off[k * S + r] * Sinv[k * S + cc];
+                        Rn[2 * S2 + r * S + cc] = a;
                     }
-                for (int r = 0; r < 3; ++r)
-                    for (int cc = 0; cc < 3; ++cc) {
-                        double a = Rn[r * 3 + cc];
-                        for (int k = 0; k < 3; ++k) a -= Rn[18 + r * 3 + k] * Off[k * 3 + cc];
-                        Sch[r * 3 + cc] = a;
+                for (int r = 0; r < S; ++r)
+                    for (int cc = 0; cc < S; ++cc) {
+                        double a = Rn[r * S + cc];
+                        for (int k = 0; k < S; ++k) a -= Rn[2 * S2 + r * S + k] * Off[k * S + cc];
+                        Sch[r * S + cc] = a;
                     }
             }
         }
@@ -190,17 +244,19 @@ PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
     return ok;
 }
 
+template <int S>
 PQP_DEV void gen_solve(Warp &w, GenCtx &cx) {
+    constexpr int RS = kGenRedStride<S>, S2 = S * S;
     const int bw = cx.bw, lane = w.lane();
     const bool act = lane < cx.M;
     const int lo = cx.lo, hi = cx.hi, gs = cx.gsep;
     const bool has_right = (lane + 1 < cx.M);
-    double *R = cx.red + (size_t)kRedStride * lane;
+    double *R = cx.red + (size_t)RS * lane;
     if (act) gen_local_solve(cx, cx.tr, lo, hi);
     w.sync();
     if (act) {
-        const int plo = lane > 0 ? cx.sep[lane - 1] + 3 : 0;
-        for (int r = 0; r < 3; ++r) {
+        const int plo = lane > 0 ? cx.sep[lane - 1] + S : 0;
+        for (int r = 0; r < S; ++r) {
             const int sg = gs + r;
             double acc = cx.tr[sg];
             if (lane > 0) {
@@ -209,28 +265,27 @@ PQP_DEV void gen_solve(Warp &w, GenCtx &cx) {
                 for (int g = g0; g < gs; ++g) acc -= PQP_GB(sg, sg - g) * cx.tr[g];
             }
             for (int g = lo; g < hi && g - sg <= bw; ++g) acc -= PQP_GB(g, g - sg) * cx.tr[g];
-            R[45 + r] = acc;
+            R[5 * S2 + r] = acc;
         }
     }
     w.sync();
     if (lane == 0) {
         for (int p = 1; p < cx.M; ++p) {
-            double *Rp = cx.red + (size_t)kRedStride * p;
-            const double *gp = Rp - kRedStride + 45;
-            for (int r = 0; r < 3; ++r)
-                Rp[45 + r] -= Rp[18 + r * 3] * gp[0] + Rp[18 + r * 3 + 1] * gp[1] + Rp[18 + r * 3 + 2] * gp[2];
+            double *Rp = cx.red + (size_t)RS * p;
+            const double *gp = Rp - RS + 5 * S2;
+            for (int r = 0; r < S; ++r) Rp[5 * S2 + r] -= gen_dot<S>(Rp + 2 * S2 + r * S, gp);
         }
-        double xn[3] = {0, 0, 0};
+        double xn[S] = {};
         for (int p = cx.M - 1; p >= 0; --p) {
-            double *Rp = cx.red + (size_t)kRedStride * p;
-            double t[3];
-            for (int r = 0; r < 3; ++r) {
-                t[r] = Rp[45 + r];
-                if (p + 1 < cx.M) t[r] -= Rp[9 + r * 3] * xn[0] + Rp[9 + r * 3 + 1] * xn[1] + Rp[9 + r * 3 + 2] * xn[2];
+            double *Rp = cx.red + (size_t)RS * p;
+            double t[S];
+            for (int r = 0; r < S; ++r) {
+                t[r] = Rp[5 * S2 + r];
+                if (p + 1 < cx.M) t[r] -= gen_dot<S>(Rp + S2 + r * S, xn);
             }
-            for (int r = 0; r < 3; ++r) xn[r] = Rp[r * 3] * t[0] + Rp[r * 3 + 1] * t[1] + Rp[r * 3 + 2] * t[2];
+            for (int r = 0; r < S; ++r) xn[r] = gen_dot<S>(Rp + r * S, t);
             const int sg = cx.sep[p];
-            cx.tr[sg] = xn[0]; cx.tr[sg + 1] = xn[1]; cx.tr[sg + 2] = xn[2];
+            for (int r = 0; r < S; ++r) cx.tr[sg + r] = xn[r];
         }
     }
     w.sync();
@@ -238,12 +293,12 @@ PQP_DEV void gen_solve(Warp &w, GenCtx &cx) {
         const int gq = hi;
         for (int g = lo; g < hi; ++g) {
             double acc = 0.0;
-            for (int r = 0; r < 3; ++r) {
+            for (int r = 0; r < S; ++r) {
                 const int sg = gs + r;
                 if (g - sg <= bw) acc -= PQP_GB(g, g - sg) * cx.tr[sg];
             }
             if (has_right)
-                for (int r = 0; r < 3; ++r) {
+                for (int r = 0; r < S; ++r) {
                     const int sg = gq + r;
                     if (sg - g <= bw) acc -= PQP_GB(sg, sg - g) * cx.tr[sg];
                 }
@@ -265,7 +320,15 @@ PQP_DEV double gen_row_dot(const GenCtx &cx, int r, const double *x) {
     return a;
 }
 
-PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int prob, double *smem, size_t smem_cap) {
+// One QP of the batch.  S: separator width (gv.sep marks S-unknown blocks).  kLinear: the cost has a linear term, q
+// [sum n] in band order at the path's n-offset, which enters OSQP's cost scaling (||c D q||), the x-step right-hand side
+// (-c q), the dual residual and its norm, and OSQP's first iteration (from x = z = y = 0 the x-step sees -c q alone and
+// z_prev = 0).  OSQP's dual-infeasibility test (q'dx < 0) is not restated: it needs a direction dx with P dx and A dx
+// both below eps_dual_inf ||dx||, which the one QP with q (pqp_smooth_reference_device's, whose every row is an
+// equality and whose P is positive definite on x, y and k) does not have for eps_dual_inf below 3e-4 (DESIGN.md §9).
+template <int S = 3, bool kLinear = false>
+PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int prob, double *smem, size_t smem_cap,
+                          const double *q = nullptr) {
     const int lane = w.lane();
     const int32_t *meta = gv.meta + (size_t)kGenMeta * prob;
     const int n = meta[0], m = meta[1], n_den = meta[2], bw = meta[3], M = meta[4], N = meta[5];
@@ -280,8 +343,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
     cx.Po_idx = gv.Po_idx + 2 * (size_t)offn; cx.Po_val = gv.Po_val + 2 * (size_t)offn;
     cx.csc_ptr = gv.csc_ptr + offp; cx.csc_row = gv.csc_row + offz; cx.csc_val = gv.csc_val + offz;
     cx.sep = gv.sep + 32 * (size_t)prob;
+    const double *qv = kLinear ? q + offn : nullptr;
     int status = PQP_UNSOLVED, iter = 0;
-    bool bad = (n < 1 || m < 1 || M < 1 || M > 32 || bw < 1 || bw > kMaxBand || gen_smem_doubles(n, m, bw) > smem_cap);
+    bool bad = (n < 1 || m < 1 || M < 1 || M > 32 || bw < 1 || bw > kMaxBand || gen_smem_doubles<S>(n, m, bw) > smem_cap);
     if (!bad) {
         double *p = smem;
         cx.D = p; p += n; cx.xr = p; p += n; cx.tr = p; p += n; cx.tmp = p; p += n; cx.sg = p; p += n;
@@ -290,7 +354,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         cx.lo = cx.hi = cx.gsep = 0;
         if (lane < M) {
             cx.gsep = cx.sep[lane];
-            cx.lo = cx.gsep + 3;
+            cx.lo = cx.gsep + S;
             cx.hi = (lane + 1 < M) ? cx.sep[lane + 1] : n;
         }
         // osqp_setup validate_data: l <= u
@@ -346,7 +410,14 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                 part += nrm;
             }
             const double mean = w.sum(part) / (double)n_den;
-            double ct = fmax(mean, 1.0);
+            double ct;
+            if constexpr (kLinear) {
+                double qn = 0.0;
+                for (int j = lane; j < n; j += 32) qn = fmax(qn, fabs(cost_c * cx.D[j] * qv[j]));
+                ct = fmax(mean, limit_scaling(w.max(qn)));
+            } else {
+                ct = fmax(mean, 1.0);
+            }
             ct = limit_scaling(ct);
             cost_c = cost_c * (1.0 / ct);
             w.sync();
@@ -356,7 +427,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         double rho = fmin(fmax(pm.rho, kRhoMin), kRhoMax);
         for (int r = lane; r < m; r += 32) cx.W[r] = rho_bar(cx.E[r] * cx.l[r], cx.E[r] * cx.u[r], rho) * cx.E[r] * cx.E[r];
         w.sync();
-        if (!gen_factor(w, cx, cost_c)) status = PQP_NON_CVX;
+        if (!gen_factor<S>(w, cx, cost_c)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
         Residuals res{};   // of the last check
         iter = 0;
@@ -365,7 +436,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
             // iterations that end in a termination check first park w = v - clamp(v): the check needs
             // delta_y = W (w_new - w_old) (OSQP update_y / is_primal_infeasible)
             const bool chk = (pm.check_termination && (iter % pm.check_termination == 0)) || iter == pm.max_iter;
-            if (iter == 1) {
+            if (iter == 1 && !kLinear) {
                 // OSQP's first iteration from x = z = y = 0 ends at the cold start (x = 0, v = 0: z = clamp(0),
                 // y = -rho clamp(0)).  Its check and rho adaptation still run below, on w_old = y_0 / rho = 0.
                 if (chk) for (int r = lane; r < m; r += 32) cx.wold[r] = 0.0;
@@ -374,17 +445,20 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                 // rhs_j = sigma_j x_j + sum_{r in col j} a_rj W_r (2 clamp(v_r) - v_r), gathered per column
                 for (int j = lane; j < n; j += 32) {
                     double acc = cx.sg[j] * cx.xr[j];
-                    for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
-                        const int r = cx.csc_row[e];
-                        const double vv = cx.v[r];
-                        acc += cx.csc_val[e] * (cx.W[r] * (2.0 * clampd(vv, cx.l[r], cx.u[r]) - vv));
-                    }
+                    if (!kLinear || iter > 1)
+                        for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
+                            const int r = cx.csc_row[e];
+                            const double vv = cx.v[r];
+                            acc += cx.csc_val[e] * (cx.W[r] * (2.0 * clampd(vv, cx.l[r], cx.u[r]) - vv));
+                        }
+                    if constexpr (kLinear) acc -= cost_c * qv[j];
                     cx.tr[j] = acc;
                 }
                 w.sync();
-                gen_solve(w, cx);
+                gen_solve<S>(w, cx);
                 for (int r = lane; r < m; r += 32) {
-                    const double vv = cx.v[r], zz = clampd(vv, cx.l[r], cx.u[r]);
+                    const double vv = cx.v[r];
+                    const double zz = (kLinear && iter == 1) ? 0.0 : clampd(vv, cx.l[r], cx.u[r]);
                     if (chk) cx.wold[r] = vv - zz;
                     cx.v[r] = vv + alpha * (gen_row_dot(cx, r, cx.tr) - zz);
                 }
@@ -402,7 +476,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                     pr = fmax(pr, fabs(rr)); nz = fmax(nz, fabs(z)); nax = fmax(nax, fabs(ax));
                     prs = fmax(prs, e * fabs(rr)); nzs = fmax(nzs, e * fabs(z)); naxs = fmax(naxs, e * fabs(ax));
                 }
-                double dr = 0, npx = 0, naty = 0, drs = 0, npxs = 0, natys = 0;
+                double dr = 0, npx = 0, naty = 0, drs = 0, npxs = 0, natys = 0, nq = 0, nqs = 0;
                 for (int j = lane; j < n; j += 32) {
                     double px = cx.Pd[j] * cx.xr[j];
                     for (int q = 0; q < 2; ++q) {
@@ -415,12 +489,22 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                         const double vv = cx.v[r];
                         aty += cx.csc_val[e] * (cx.W[r] * (vv - clampd(vv, cx.l[r], cx.u[r])) * cinv);
                     }
-                    const double rr = px + aty, cd = cost_c * cx.D[j];
+                    double rr = px + aty;
+                    const double cd = cost_c * cx.D[j];
+                    if constexpr (kLinear) {
+                        rr = qv[j] + px + aty;
+                        nq = fmax(nq, fabs(qv[j]));
+                        nqs = fmax(nqs, cd * fabs(qv[j]));
+                    }
                     dr = fmax(dr, fabs(rr)); npx = fmax(npx, fabs(px)); naty = fmax(naty, fabs(aty));
                     drs = fmax(drs, cd * fabs(rr)); npxs = fmax(npxs, cd * fabs(px)); natys = fmax(natys, cd * fabs(aty));
                 }
                 pr = w.max(pr); nz = w.max(nz); nax = w.max(nax); prs = w.max(prs); nzs = w.max(nzs); naxs = w.max(naxs);
                 dr = w.max(dr); npx = w.max(npx); naty = w.max(naty); drs = w.max(drs); npxs = w.max(npxs); natys = w.max(natys);
+                if constexpr (kLinear) {
+                    nq = w.max(nq); nqs = w.max(nqs);
+                    npx = fmax(npx, nq); npxs = fmax(npxs, nqs);   // OSQP's dual norm: max(||q||, ||Px||, ||A'y||)
+                }
                 w.sync();
                 // ---- primal-infeasibility certificate (OSQP is_primal_infeasible) in unscaled terms:
                 // g = W (w_new - w_old) = E delta_y projected on the cone of the finite (scaled) bounds;
@@ -461,7 +545,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                         }
                         rho = rho_new;
                         w.sync();
-                        if (!gen_factor(w, cx, cost_c)) status = PQP_NON_CVX;
+                        if (!gen_factor<S>(w, cx, cost_c)) status = PQP_NON_CVX;
                     }
                 }
             }

@@ -34,4 +34,5 @@ PQP_DECLARE_VARIANT(kk_13)
 // one-warp generic KP kernel (any keep <= 10) and the generic banded-QP kernel of "K" / "KPC"
 PQP_DECLARE_VARIANT(k1_generic)
 const void *pqp_gen_kernel_fn();
+const void *pqp_gen4_kernel_fn();    // the same core with 4-unknown separators and a linear cost (pqp_kgen4.cu)
 void pqp_k1_set_smem_cap(int bytes);   // device's opt-in shared memory per block (decides where the one-warp kernel keeps its scalings)

@@ -388,6 +388,44 @@ class PathPlanner(BatchPathSolver):
         return dict(knot_offsets=ko, knots=kn, x_coef=xc, y_coef=yc, max_s=ms, ok=ok, status=status, iters=iters,
                     layers=layers)
 
+    def smooth_device(self, points, point_offsets, max_raw_samples, max_points, capacity=None, weights=(0.005, 1, 10),
+                      out=None):
+        """ReferencePathSmoother's B-spline pre-pass and TENSION2 smoothing QP for every raw polyline of a batch on the
+        device (pqp_smooth_reference_device): raw polylines in, smoothed lines out in the layout post_smooth_device
+        reads as `splines`.  points float64 [P, 7] (x and y read), point_offsets int32 [B + 1], torch CUDA tensors; on
+        torch.cuda.current_stream().  max_raw_samples: B-spline samples a path may have at most; max_points: stations
+        a path may have at most; capacity: knot rows of the output (default the planner's max_total_points); weights:
+        FLAGS_tension_2_deviation_weight, _curvature_weight, _curvature_rate_weight.  Returns dict(knot_offsets int32
+        [B + 1], knots [capacity], x_coef / y_coef [capacity, 4], max_s [B], ok, status, iters int32 [B]).  A refused
+        path gets ok = 0, 0 knots and NaN max_s.  No host synchronisation; after one call with the largest caps it can
+        be captured in a CUDA graph.  `out` may carry the output tensors, e.g. those of an earlier call."""
+        import torch
+        from . import device as D
+        dev = self._cuda_device()
+        B = int(point_offsets.shape[0]) - 1
+        P = int(points.shape[0])
+        cap = int(self.max_total_points if capacity is None else capacity)
+        f64, i32 = torch.float64, torch.int32
+        out = dict(out or {})
+
+        def buf(name, shp, dtype):
+            return out[name] if out.get(name) is not None else torch.empty(shp, dtype=dtype, device=dev)
+        ko, kn = buf("knot_offsets", (B + 1,), i32), buf("knots", (cap,), f64)
+        xc, yc, ms = buf("x_coef", (cap, 4), f64), buf("y_coef", (cap, 4), f64), buf("max_s", (B,), f64)
+        ok, status, iters = buf("ok", (B,), i32), buf("status", (B,), i32), buf("iters", (B,), i32)
+        w_dev, w_curv, w_rate = (float(v) for v in weights)
+        rc = self._L.pqp_smooth_reference_device(
+            self._h, B, D.check(point_offsets, "point_offsets", i32, (B + 1,), dev),
+            D.check(points, "points", f64, (P, D.STATE_COLS), dev), w_dev, w_curv, w_rate, int(max_raw_samples),
+            int(max_points), cap, D.check(ko, "knot_offsets", i32, (B + 1,), dev), D.check(kn, "knots", f64, (cap,), dev),
+            D.check(xc, "x_coef", f64, (cap, 4), dev), D.check(yc, "y_coef", f64, (cap, 4), dev),
+            D.check(ms, "max_s", f64, (B,), dev), D.check(ok, "ok", i32, (B,), dev),
+            D.check(status, "status", i32, (B,), dev), D.check(iters, "iters", i32, (B,), dev),
+            torch.cuda.current_stream(dev).cuda_stream)
+        if rc != OK:
+            raise PqpError(f"pqp_smooth_reference_device failed (rc={rc}): {_lib.last_error()}")
+        return dict(knot_offsets=ko, knots=kn, x_coef=xc, y_coef=yc, max_s=ms, ok=ok, status=status, iters=iters)
+
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
                     bounds_mode=BOUNDS_SIMPLE, splines=None, output_mode=OUTPUT_RAW, output_spacing=0.3,
                     collision_check=True, max_out=512, want_bounds=False, out=None, stats=False, map_index=None,
