@@ -108,11 +108,14 @@ enum pqp_formulation {
  * At max_iter, when the last check has not stopped the run, OSQP 0.6 checks once more with eps_abs, eps_rel and
  * eps_prim_inf x 10: PQP_SOLVED_INACCURATE when the residuals pass, PQP_PRIMAL_INFEASIBLE_INACCURATE when the
  * infeasibility certificate holds, else PQP_MAX_ITER_REACHED.  PQP_SOLVED_INACCURATE and PQP_MAX_ITER_REACHED carry
- * the last iterate; PQP_PRIMAL_INFEASIBLE and PQP_PRIMAL_INFEASIBLE_INACCURATE carry NaN. */
+ * the last iterate; PQP_PRIMAL_INFEASIBLE and PQP_PRIMAL_INFEASIBLE_INACCURATE carry NaN.  Only a QP with a linear
+ * cost term (the smoothing QP of pqp_smooth_reference_device) can be dual infeasible: PQP_DUAL_INFEASIBLE, or
+ * PQP_DUAL_INFEASIBLE_INACCURATE in the x10 re-check (eps_dual_inf x 10 as well); both carry NaN. */
 enum pqp_status {
     PQP_SOLVED                 = 1,
     PQP_SOLVED_INACCURATE      = 2,
     PQP_PRIMAL_INFEASIBLE_INACCURATE = 3,
+    PQP_DUAL_INFEASIBLE_INACCURATE = 4,
     PQP_MAX_ITER_REACHED       = -2,
     PQP_PRIMAL_INFEASIBLE      = -3,
     PQP_DUAL_INFEASIBLE        = -4,

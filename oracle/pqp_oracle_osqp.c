@@ -422,6 +422,7 @@ typedef struct {
     double rho;
     double *x, *z, *y, *x_prev, *z_prev, *xz_tilde, *rhs;
     double *Ax, *Px, *Aty, *delta_x, *delta_y, *Adelta_x, *Atdelta_y, *Pdelta_x;
+    int has_q;   /* q != 0: only then can the dual-infeasibility test fire, and only then are its margins noted */
     double *D_temp, *D_temp_A, *E_temp;
     double margin;         /* smallest relative gap of a value from its threshold in the checks since the last reset */
 } work;
@@ -589,14 +590,26 @@ static int is_dual_infeasible(work *w, double eps_dual_inf) {
     const int m = w->m, n = w->n;
     double norm_delta_x = vec_scaled_norm_inf(w->D, w->delta_x, n);
     double cost_scaling = w->c;
+    if (!w->has_q) return 0;   /* q'dx = 0 is never below -eps ||dx|| c */
+    note_gap(w, norm_delta_x, eps_dual_inf);
     if (norm_delta_x > eps_dual_inf) {
         double qdx = 0;
         for (int i = 0; i < n; ++i) qdx += w->q[i] * w->delta_x[i];
+        note_gap(w, qdx, -cost_scaling * eps_dual_inf * norm_delta_x);
         if (qdx < -cost_scaling * eps_dual_inf * norm_delta_x) {
             sym_triu_vec(w->P, w->delta_x, w->Pdelta_x);
-            if (vec_scaled_norm_inf(w->Dinv, w->Pdelta_x, n) < cost_scaling * eps_dual_inf * norm_delta_x) {
+            const double pdx = vec_scaled_norm_inf(w->Dinv, w->Pdelta_x, n);
+            note_gap(w, pdx, cost_scaling * eps_dual_inf * norm_delta_x);
+            if (pdx < cost_scaling * eps_dual_inf * norm_delta_x) {
                 mat_vec(w->A, w->delta_x, w->Adelta_x);
                 for (int i = 0; i < m; ++i) w->Adelta_x[i] *= w->Einv[i];
+                double up = -INFINITY, lo = -INFINITY;   /* the rows closest to breaking the certificate */
+                for (int i = 0; i < m; ++i) {
+                    if (w->u[i] < OSQP_INFTY * MIN_SCALING) up = c_max(up, w->Adelta_x[i]);
+                    if (w->l[i] > -OSQP_INFTY * MIN_SCALING) lo = c_max(lo, -w->Adelta_x[i]);
+                }
+                if (up > -INFINITY) note_gap(w, up, eps_dual_inf * norm_delta_x);
+                if (lo > -INFINITY) note_gap(w, lo, eps_dual_inf * norm_delta_x);
                 for (int i = 0; i < m; ++i) {
                     if (((w->u[i] < OSQP_INFTY * MIN_SCALING) && (w->Adelta_x[i] > eps_dual_inf * norm_delta_x)) ||
                         ((w->l[i] > -OSQP_INFTY * MIN_SCALING) && (w->Adelta_x[i] < -eps_dual_inf * norm_delta_x)))
@@ -630,7 +643,7 @@ static int check_termination(work *w, const pqp_params *prm, double pri_res, dou
     else dual_inf_check = is_dual_infeasible(w, eps_dual_inf);
     if (prim_res_check && dual_res_check) { *status = approximate ? PQP_SOLVED_INACCURATE : PQP_SOLVED; return 1; }
     if (prim_inf_check) { *status = approximate ? PQP_PRIMAL_INFEASIBLE_INACCURATE : PQP_PRIMAL_INFEASIBLE; return 1; }
-    if (dual_inf_check) { *status = PQP_DUAL_INFEASIBLE; return 1; }
+    if (dual_inf_check) { *status = approximate ? PQP_DUAL_INFEASIBLE_INACCURATE : PQP_DUAL_INFEASIBLE; return 1; }
     return 0;
 }
 
@@ -684,6 +697,7 @@ int oracle_osqp_solve(const pqp_params *prm, const oqp_problem *qp, double *x_ou
     int *a_map = triplet_to_csc_map(n, qp->a_nnz, qp->a_j);
     w->q = dalloc(n); w->l = dalloc(m); w->u = dalloc(m);
     memcpy(w->q, qp->q, sizeof(double) * (size_t)n);
+    for (int i = 0; i < n; ++i) w->has_q |= qp->q[i] != 0.0;
     memcpy(w->l, qp->l, sizeof(double) * (size_t)m);
     memcpy(w->u, qp->u, sizeof(double) * (size_t)m);
     w->D = dalloc(n); w->Dinv = dalloc(n); w->E = dalloc(m); w->Einv = dalloc(m);

@@ -19,6 +19,7 @@ FORMULATIONS = {"KP": FORM_KP, "K": FORM_K, "KPC": FORM_KPC}
 SOLVED = 1
 SOLVED_INACCURATE = 2
 PRIMAL_INFEASIBLE_INACCURATE = 3
+DUAL_INFEASIBLE_INACCURATE = 4
 MAX_ITER_REACHED = -2
 PRIMAL_INFEASIBLE = -3
 DUAL_INFEASIBLE = -4

@@ -123,7 +123,8 @@ struct Residuals {
 };
 
 // OSQP check_termination (unscaled residuals, strict <): PQP_NON_CVX, PQP_SOLVED,
-// PQP_PRIMAL_INFEASIBLE or PQP_UNSOLVED.  q = 0, so the dual-infeasibility test (q'dx < 0) never fires.
+// PQP_PRIMAL_INFEASIBLE or PQP_UNSOLVED.  The dual-infeasibility test (q'dx < 0) is not here: with q = 0 it never
+// fires, and the one core with a linear term (gen_solve_qp<4, true>, pqp_gen_core.cuh) adds it after this call.
 PQP_DEV int termination_verdict(const DevParams &pm, const Residuals &r) {
     const bool prim_ok = r.pri_res < pm.eps_abs + pm.eps_rel * r.pri_nrm;
     if (r.pri_res > kOsqpInfty || r.dua_res > kOsqpInfty) return PQP_NON_CVX;

@@ -41,7 +41,7 @@ struct GenView {
     int32_t *status, *iters; // [B]
 };
 
-// Per-lane reduction record of an S-wide separator: [0, S^2) Dg / Sinv, [S^2, 2S^2) Off, [2S^2, 3S^2) G,
+// Per-lane reduction record of an S-wide separator: [0, S^2) Dg / Sinv (S = 3) or its LDL' factors (S = 4), [S^2, 2S^2) Off, [2S^2, 3S^2) G,
 // [3S^2, 4S^2) A, [4S^2, 5S^2) C, [5S^2, 5S^2 + S) g.  S = 3 gives kRedStride.
 template <int S> constexpr int kGenRedStride = 5 * S * S + S;
 static_assert(kGenRedStride<3> == kRedStride, "width-3 record");
@@ -51,36 +51,38 @@ PQP_HD size_t gen_smem_doubles(int n, int m, int bw) {
     return 5 * (size_t)n + 4 * (size_t)m + (size_t)(bw + 1) * n + (size_t)kGenRedStride<S> * 32;
 }
 
-// Inverse of an SPD S x S block (row-major), S = 3 through inv3_spd, S = 4 by LDL'.
-template <int S> PQP_DEV void gen_inv_spd(const double *a, double *o) {
-    if constexpr (S == 3) {
-        inv3_spd(a, o);
-    } else {
-        double L[S * S], d[S];
-        for (int j = 0; j < S; ++j) {
-            double dj = a[j * S + j];
-            for (int k = 0; k < j; ++k) dj -= L[j * S + k] * L[j * S + k] * d[k];
-            d[j] = dj;
-            for (int i = j + 1; i < S; ++i) {
-                double v = a[i * S + j];
-                for (int k = 0; k < j; ++k) v -= L[i * S + k] * L[j * S + k] * d[k];
-                L[i * S + j] = v / dj;
-            }
+// LDL' of an SPD S x S block a (row-major) into f: the unit lower factor below the diagonal, 1 / d on it.  The width-4
+// separator chain keeps these factors and solves with them: an explicit inverse of its Schur blocks, which are far worse
+// conditioned than the QP's KKT system when the cost scaling c is small (UTM-sized coordinates, a large deviation
+// weight), loses up to all digits of the x-step there (DESIGN.md §9).
+template <int S> PQP_DEV void gen_ldl_spd(const double *a, double *f) {
+    double d[S];
+    for (int j = 0; j < S; ++j) {
+        double dj = a[j * S + j];
+        for (int k = 0; k < j; ++k) dj -= f[j * S + k] * f[j * S + k] * d[k];
+        d[j] = dj;
+        const double rj = 1.0 / dj;
+        f[j * S + j] = rj;
+        for (int i = j + 1; i < S; ++i) {
+            double v = a[i * S + j];
+            for (int k = 0; k < j; ++k) v -= f[i * S + k] * f[j * S + k] * d[k];
+            f[i * S + j] = v * rj;
         }
-        // inv = L^-T diag(1/d) L^-1, column c of L^-1 by forward substitution
-        double Mi[S * S];
-        for (int c = 0; c < S; ++c)
-            for (int i = 0; i < S; ++i) {
-                double v = i == c ? 1.0 : 0.0;
-                for (int k = c; k < i; ++k) v -= L[i * S + k] * Mi[k * S + c];
-                Mi[i * S + c] = v;
-            }
-        for (int r = 0; r < S; ++r)
-            for (int c = r; c < S; ++c) {
-                double v = 0.0;
-                for (int k = c; k < S; ++k) v += Mi[k * S + r] * Mi[k * S + c] / d[k];
-                o[r * S + c] = o[c * S + r] = v;
-            }
+    }
+}
+// x = (L D L')^-1 b for the factors of gen_ldl_spd (x may alias b).
+template <int S> PQP_DEV void gen_ldl_solve(const double *f, const double *b, double *x) {
+    double y[S];
+    for (int i = 0; i < S; ++i) {
+        double v = b[i];
+        for (int k = 0; k < i; ++k) v -= f[i * S + k] * y[k];
+        y[i] = v;
+    }
+    for (int i = 0; i < S; ++i) y[i] *= f[i * S + i];
+    for (int i = S - 1; i >= 0; --i) {
+        double v = y[i];
+        for (int k = i + 1; k < S; ++k) v -= f[k * S + i] * x[k];
+        x[i] = v;
     }
 }
 
@@ -219,17 +221,30 @@ PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
         for (int p = 0; p < cx.M; ++p) {
             double *Rp = cx.red + (size_t)RS * p;
             if (!(Sch[0] > 0.0)) ok = 0;
-            gen_inv_spd<S>(Sch, Sinv);
-            for (int k = 0; k < S2; ++k) Rp[k] = Sinv[k];
+            if constexpr (S == 3) {
+                inv3_spd(Sch, Sinv);
+                for (int k = 0; k < S2; ++k) Rp[k] = Sinv[k];
+            } else {
+                gen_ldl_spd<S>(Sch, Rp);   // Dg holds the block's LDL' factors (gen_solve solves with them)
+            }
             if (p + 1 < cx.M) {
                 double *Rn = Rp + RS;
                 const double *Off = Rp + S2;
-                for (int r = 0; r < S; ++r)
-                    for (int cc = 0; cc < S; ++cc) {
-                        double a = 0.0;
-                        for (int k = 0; k < S; ++k) a += Off[k * S + r] * Sinv[k * S + cc];
-                        Rn[2 * S2 + r * S + cc] = a;
+                if constexpr (S == 3) {
+                    for (int r = 0; r < S; ++r)
+                        for (int cc = 0; cc < S; ++cc) {
+                            double a = 0.0;
+                            for (int k = 0; k < S; ++k) a += Off[k * S + r] * Sinv[k * S + cc];
+                            Rn[2 * S2 + r * S + cc] = a;
+                        }
+                } else {
+                    // row r of G = column r of Off solved against the block
+                    for (int r = 0; r < S; ++r) {
+                        double o[S];
+                        for (int k = 0; k < S; ++k) o[k] = Off[k * S + r];
+                        gen_ldl_solve<S>(Rp, o, Rn + 2 * S2 + r * S);
                     }
+                }
                 for (int r = 0; r < S; ++r)
                     for (int cc = 0; cc < S; ++cc) {
                         double a = Rn[r * S + cc];
@@ -283,7 +298,11 @@ PQP_DEV void gen_solve(Warp &w, GenCtx &cx) {
                 t[r] = Rp[5 * S2 + r];
                 if (p + 1 < cx.M) t[r] -= gen_dot<S>(Rp + S2 + r * S, xn);
             }
-            for (int r = 0; r < S; ++r) xn[r] = gen_dot<S>(Rp + r * S, t);
+            if constexpr (S == 3) {
+                for (int r = 0; r < S; ++r) xn[r] = gen_dot<S>(Rp + r * S, t);
+            } else {
+                gen_ldl_solve<S>(Rp, t, xn);
+            }
             const int sg = cx.sep[p];
             for (int r = 0; r < S; ++r) cx.tr[sg + r] = xn[r];
         }
@@ -320,12 +339,20 @@ PQP_DEV double gen_row_dot(const GenCtx &cx, int r, const double *x) {
     return a;
 }
 
+// OSQP is_dual_infeasible on the certificate (||dx||, q'dx, ||P dx||, max A dx over rows with a finite upper bound,
+// max -A dx over rows with a finite lower bound), in unscaled terms.
+PQP_DEV bool dual_infeasible(double nrm, double qdx, double pdx, double adx_up, double adx_lo, double eps) {
+    return nrm > eps && qdx < -eps * nrm && pdx < eps * nrm && adx_up <= eps * nrm && adx_lo <= eps * nrm;
+}
+
 // One QP of the batch.  S: separator width (gv.sep marks S-unknown blocks).  kLinear: the cost has a linear term, q
 // [sum n] in band order at the path's n-offset, which enters OSQP's cost scaling (||c D q||), the x-step right-hand side
-// (-c q), the dual residual and its norm, and OSQP's first iteration (from x = z = y = 0 the x-step sees -c q alone and
-// z_prev = 0).  OSQP's dual-infeasibility test (q'dx < 0) is not restated: it needs a direction dx with P dx and A dx
-// both below eps_dual_inf ||dx||, which the one QP with q (pqp_smooth_reference_device's, whose every row is an
-// equality and whose P is positive definite on x, y and k) does not have for eps_dual_inf below 3e-4 (DESIGN.md §9).
+// (-c q), the dual residual and its norm, OSQP's first iteration (from x = z = y = 0 the x-step sees -c q alone and
+// z_prev = 0), and OSQP's dual-infeasibility test (is_dual_infeasible: the step dx of a check iteration with
+// q'dx < -eps ||dx||, ||P dx|| < eps ||dx|| and A dx within eps ||dx|| of the recession cone of the bounds, all in
+// unscaled terms, eps = eps_dual_inf).  It runs after the SOLVED and primal-infeasibility tests, when the dual residual
+// fails, in the exact check (PQP_DUAL_INFEASIBLE) and in the x10 re-check at max_iter (PQP_DUAL_INFEASIBLE_INACCURATE).
+// dx is parked in tmp, which gen_solve leaves free until the next solve.  With q = 0, q'dx < 0 never holds.
 template <int S = 3, bool kLinear = false>
 PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int prob, double *smem, size_t smem_cap,
                           const double *q = nullptr) {
@@ -430,6 +457,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         if (!gen_factor<S>(w, cx, cost_c)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
         Residuals res{};   // of the last check
+        // dual-infeasibility certificate of the last check (kLinear), at eps_dual_inf and at 10 eps_dual_inf
+        bool di_1 = false, di_10 = false;
+        (void)di_1; (void)di_10;
         iter = 0;
         while (status == PQP_UNSOLVED && iter < pm.max_iter) {
             ++iter;
@@ -462,7 +492,15 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                     if (chk) cx.wold[r] = vv - zz;
                     cx.v[r] = vv + alpha * (gen_row_dot(cx, r, cx.tr) - zz);
                 }
-                for (int j = lane; j < n; j += 32) cx.xr[j] = alpha * cx.tr[j] + (1.0 - alpha) * cx.xr[j];
+                if constexpr (kLinear) {
+                    for (int j = lane; j < n; j += 32) {
+                        const double xn = alpha * cx.tr[j] + (1.0 - alpha) * cx.xr[j];
+                        if (chk) cx.tmp[j] = xn - cx.xr[j];
+                        cx.xr[j] = xn;
+                    }
+                } else {
+                    for (int j = lane; j < n; j += 32) cx.xr[j] = alpha * cx.tr[j] + (1.0 - alpha) * cx.xr[j];
+                }
             }
             w.sync();
             const bool can_check = pm.check_termination && (iter % pm.check_termination == 0);
@@ -531,8 +569,37 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                     res.inf_nrm = w.max(c_nrm); res.inf_cert = w.max(c_cert); res.inf_lhs = w.sum(c_lhs);
                     w.sync();
                 }
+                if constexpr (kLinear) {
+                    if (chk) {
+                        double dn = 0, qd = 0, pd = 0, au = -INFINITY, al = -INFINITY;
+                        for (int j = lane; j < n; j += 32) {
+                            const double dx = cx.tmp[j];
+                            double p = cx.Pd[j] * dx;
+                            for (int q = 0; q < 2; ++q) {
+                                const int k = cx.Po_idx[2 * j + q];
+                                if (k >= 0) p += cx.Po_val[2 * j + q] * cx.tmp[k];
+                            }
+                            dn = fmax(dn, fabs(dx)); qd += qv[j] * dx; pd = fmax(pd, fabs(p));
+                        }
+                        for (int r = lane; r < m; r += 32) {
+                            const double ad = gen_row_dot(cx, r, cx.tmp);
+                            if (cx.E[r] * cx.u[r] < kOsqpInfty * kMinScaling) au = fmax(au, ad);
+                            if (cx.E[r] * cx.l[r] > -kOsqpInfty * kMinScaling) al = fmax(al, -ad);
+                        }
+                        dn = w.max(dn); qd = w.sum(qd); pd = w.max(pd); au = w.max(au); al = w.max(al);
+                        di_1 = dual_infeasible(dn, qd, pd, au, al, pm.eps_dual_inf);
+                        di_10 = dual_infeasible(dn, qd, pd, au, al, 10 * pm.eps_dual_inf);
+                        w.sync();
+                    }
+                }
                 res.pri_res = pr; res.dua_res = dr; res.pri_nrm = fmax(nz, nax); res.dua_nrm = fmax(npx, naty);
-                if (can_check || iter == pm.max_iter) status = termination_verdict(pm, res);
+                if (can_check || iter == pm.max_iter) {
+                    status = termination_verdict(pm, res);
+                    if constexpr (kLinear)
+                        if (status == PQP_UNSOLVED && !(res.dua_res < pm.eps_abs + pm.eps_rel * res.dua_nrm) &&
+                            di_1)
+                            status = PQP_DUAL_INFEASIBLE;
+                }
                 if (status == PQP_UNSOLVED && can_adapt) {
                     const double rho_new = rho_estimate(rho, prs, drs, fmax(nzs, naxs), fmax(npxs, natys));
                     if (rho_changed(pm, rho_new, rho)) {
@@ -550,7 +617,13 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                 }
             }
         }
-        if (status == PQP_UNSOLVED) status = max_iter_verdict(pm, res);
+        if (status == PQP_UNSOLVED) {
+            status = max_iter_verdict(pm, res);
+            if constexpr (kLinear)
+                if (status == PQP_MAX_ITER_REACHED && !(res.dua_res < 10 * pm.eps_abs + 10 * pm.eps_rel * res.dua_nrm) &&
+                    di_10)
+                    status = PQP_DUAL_INFEASIBLE_INACCURATE;
+        }
     }
     // ---- epilogue: getOptimizedPath (solver_k_as_input.cpp:22-44, ..._constrained.cpp:26-43)
     const bool has_sol = has_solution(status);
