@@ -307,7 +307,8 @@ int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offse
  * y_0, solved with the handle's OSQP settings (the reference's OsqpEigen solver sets only verbosity and warm start, so
  * under the default settings these are the settings it runs with); and TensionSmoother::smooth's tail
  * (tension_smoother.cpp:84-96) -- s accumulated from the solution's x, y, the natural splines x(s), y(s) fitted through
- * them, max_s = s.back() + 3.  The IPOPT solver and the TENSION and ANGLE_DIFF methods are not restated.
+ * them, max_s = s.back() + 3.  The TENSION method is pqp_smooth_reference_tension_device below; the IPOPT solver and
+ * the ANGLE_DIFF method are not restated.
  * A path is refused (ok = 0, 0 knots, NaN max_s; no other path changes) when:
  *   - it has fewer than 4 points (:36-39);
  *   - the B-spline's degree is not below its point count (tinyspline refuses such a spline and the reference throws;
@@ -332,6 +333,34 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
                                 int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
                                 double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
                                 int32_t *d_status, int32_t *d_iters, void *stream);
+
+/* pqp_smooth_reference_device with smoothing_method TENSION (tension_solver OSQP): the same B-spline pre-pass,
+ * segmentRawReference, tail, outputs and reservation, with TensionSmoother's clearance-bounded smoothing QP in place of
+ * TensionSmoother2's.  Parameters as pqp_smooth_reference_device, plus
+ *   deviation_w, curvature_w, curvature_rate_w   FLAGS_cartesian_deviation_weight, _curvature_weight and
+ *                      _curvature_rate_weight (0, 1, 50)
+ *   d_map_index        [batch] the map of every path in the handle's map set (pqp_set_map / pqp_set_maps), or NULL for
+ *                      map 0
+ * Per path, TensionSmoother::osqpSmooth (tension_smoother.cpp:186-237) with setHessianMatrix (:239-263) and
+ * setConstraintMatrix (:265-314): over the N stations (x_i, y_i, heading_i) of segmentRawReference, the unknowns x_i,
+ * y_i and the lateral offsets d_i; q = 0; P the dds blocks (1, -2, 1)(1, -2, 1)' curvature_w and the ddds blocks
+ * (-1, 3, -3, 1)(-1, 3, -3, 1)' curvature_rate_w of the x and y chains, and deviation_w on every d_i; the rows
+ * x_i - cos(theta_i) d_i = x_ref_i, y_i - sin(theta_i) d_i = y_ref_i with theta_i = heading_i + pi/2, and d_i with
+ * d_0 = 0, |d_{N-1}| <= 0.5 and |d_i| <= min(clearance_i, 2) between, clearance_i being Map::getObstacleDistance
+ * (Map.cpp:16-22) at the station in the path's map (bilinear in the distance layer, 0 outside the map); exact zeros of
+ * P and A dropped as Eigen's sparseView drops them; solved with the handle's OSQP settings.  The smoothed line is the
+ * solution's x_i, y_i, followed by TensionSmoother::smooth's tail (:84-96) as above.
+ * A path is refused for the reasons of pqp_smooth_reference_device, and when its map index lies outside the map set.
+ * Errors as pqp_smooth_reference_device, and PQP_ERR_ARG when the handle has no map set; the QP fits one SM's shared
+ * memory up to 277 stations on an H100 (227 KB), so a larger max_points returns PQP_ERR_CAPACITY.  The scratch is the
+ * smoothing stage's, sized for whichever of the two QPs asked for more.
+ * Replaces: ReferencePathSmoother::bSpline + TensionSmoother::smooth (TENSION, OSQP), once per path. */
+int pqp_smooth_reference_tension_device(pqp_handle *h, int batch, const int32_t *d_point_offsets,
+                                        const pqp_state *d_points, double deviation_w, double curvature_w,
+                                        double curvature_rate_w, const int32_t *d_map_index, int max_raw_samples,
+                                        int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
+                                        double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
+                                        int32_t *d_status, int32_t *d_iters, void *stream);
 
 /* tk::spline::operator() / deriv (spline.cpp:250-318) on a fitted spline; order 0..2. */
 double pqp_spline_eval(int n, const double *t, const double *coef, int order, double at);

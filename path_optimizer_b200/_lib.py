@@ -22,7 +22,7 @@ ENV_SYMBOLS = ["pqp_update_limits", "pqp_update_limits_device", "pqp_set_map", "
                "pqp_plan_batch_device_sets", "pqp_set_maps_occupancy", "pqp_set_maps_occupancy_device", "pqp_get_map",
                "pqp_plan_batch_forms", "pqp_plan_batch_device_forms", "pqp_fit_splines_device",
                "pqp_segment_reference_device", "pqp_post_smooth_device",
-               "pqp_smooth_reference_device"]
+               "pqp_smooth_reference_device", "pqp_smooth_reference_tension_device"]
 # ... and include/pqp_multi.h
 MULTI_SYMBOLS = ["pqp_nccl_unique_id", "pqp_comm_init_rank", "pqp_allgather", "pqp_comm_destroy", "pqp_multi_create",
                  "pqp_multi_destroy", "pqp_multi_devices", "pqp_multi_solve_batch", "pqp_multi_gathered",
@@ -108,6 +108,8 @@ def load():
                                                 C.c_int, C.c_int] + [vp] * 7)
     L.pqp_post_smooth_device.argtypes = ([vp, C.c_int] + [vp] * 7 + [C.c_double] * 3 + [C.c_int, C.c_int] + [vp] * 10)
     L.pqp_smooth_reference_device.argtypes = ([vp, C.c_int, vp, vp] + [C.c_double] * 3 + [C.c_int] * 3 + [vp] * 9)
+    L.pqp_smooth_reference_tension_device.argtypes = ([vp, C.c_int, vp, vp] + [C.c_double] * 3 + [vp] + [C.c_int] * 3 +
+                                                      [vp] * 9)
     # include/pqp_multi.h
     L.pqp_nccl_unique_id.argtypes = [vp]
     L.pqp_comm_init_rank.argtypes = [vp, C.c_int, C.c_int, vp]

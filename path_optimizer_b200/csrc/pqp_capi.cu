@@ -822,6 +822,7 @@ int pqp_create(pqp_handle **out, const pqp_params *params, int device, int max_b
         PQP_TRY(cudaFuncSetAttribute(kVariants[v].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     PQP_TRY(cudaFuncSetAttribute(pqp_gen_kernel_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     PQP_TRY(cudaFuncSetAttribute(pqp_gen4_kernel_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
+    PQP_TRY(cudaFuncSetAttribute(pqp_gen9_kernel_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin));
     PQP_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     PQP_TRY(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
     for (auto &e : h->ev_chunk) PQP_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));

@@ -749,6 +749,9 @@ pqp_corridor_copy_kernel(const __grid_constant__ CorridorArgs a) {
 // accumulates s and keeps the path when its QP is SOLVED and s strictly increasing; (6) the segment stage's one-warp
 // reservation; (7) one thread per kept path copies its points to their reserved rows; (8) pqp_fit_splines_kernel fits
 // x(s), y(s).  Between the launches the per-path state sits in the handle's scratch, at fixed strides.
+// pqp_smooth_reference_tension_device runs the same launches with two replaced: (3) assembles the TENSION QP
+// (pqp_smooth_tension_assemble_kernel, which also looks each station's clearance up in the path's map) and (4) solves it
+// with pqp_gen9_solve_kernel.
 struct SmoothArgs {
     pqp::SmoothWeights w;
     int batch, max_raw, max_points;
@@ -849,6 +852,72 @@ pqp_smooth_assemble_kernel(const __grid_constant__ SmoothArgs a) {
         for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;
         mb[0] = 4 * N - 1; mb[1] = 3 * N - 1; mb[2] = 4 * N - 1; mb[3] = 4; mb[4] = M; mb[5] = N;
         mb[6] = (int32_t)oN; mb[7] = (int32_t)on; mb[8] = (int32_t)om; mb[9] = (int32_t)oz; mb[10] = (int32_t)op;
+    }
+}
+
+// The front of pqp_smooth_assemble_kernel for the TENSION assemble kernel: a path whose raw fit failed or whose station
+// count lies outside [3, max_points] gets its refusal and 0; otherwise returns its station count N and its raw splines.
+// (pqp_smooth_assemble_kernel keeps these lines inline: calling this changes its register allocation.)
+__device__ __forceinline__ int smooth_front(const SmoothArgs &a, int b, SplineView *xs, SplineView *ys) {
+    const int Km = a.max_raw, Nm = a.max_points;
+    if (!a.raw_ok[2 * b]) { smooth_refuse(a, b, pqp::SM_RAW_ORDER); return 0; }
+    const int K = a.raw_off[2 * b + 1] - a.raw_off[2 * b];
+    const size_t ro = (size_t)b * Km;
+    *xs = SplineView{K, a.raw_knots + ro, a.raw_xc + 4 * ro};
+    *ys = SplineView{K, a.raw_knots + ro, a.raw_yc + 4 * ro};
+    const double max_s = a.raw_knots[ro + K - 1];
+    if (!(max_s <= (double)Nm)) { smooth_refuse(a, b, pqp::SM_MANY); return 0; }
+    const int N = pqp::smooth_station_count(max_s);
+    if (N > Nm) { smooth_refuse(a, b, pqp::SM_MANY); return 0; }
+    if (N < 3) { smooth_refuse(a, b, pqp::SM_SHORT); return 0; }
+    return N;
+}
+
+// (3) of pqp_smooth_reference_tension_device: a path whose map index lies outside the map set is refused, then the
+// stations as above, each with its clearance (Map::getObstacleDistance at the station) and the TENSION QP in band order.
+// A station's CSC entries start after those of the stations before it: a warp scan per 32 stations.
+__global__ void __launch_bounds__(32)
+pqp_smooth_tension_assemble_kernel(const __grid_constant__ SmoothArgs a, const MapTable maps) {
+    const int b = blockIdx.x, lane = threadIdx.x, Nm = a.max_points;
+    if (a.reason[b] != pqp::SM_OK) return;
+    const MapView *mp = pqp::map_of(maps, b);
+    if (!mp) return smooth_refuse(a, b, pqp::SM_MAP);
+    SplineView xs, ys;
+    const int N = smooth_front(a, b, &xs, &ys);
+    if (N == 0) return;
+    const MapView m = *mp;
+    constexpr int P = pqp::kTensionPartners;
+    const size_t oN = (size_t)b * Nm, on = 3 * oN, oz = 5 * oN, op = (size_t)b * (3 * Nm + 1);
+    int e0 = 0;
+    for (int i0 = 0; i0 < N; i0 += 32) {
+        const int i = i0 + lane;
+        pqp_state st{};
+        int cnt = 0;
+        if (i < N) {
+            st = pqp::densify_sample(xs, ys, (double)i);
+            cnt = pqp::tension_qp_csc_count(st);
+        }
+        int incl = cnt;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (i < N) {
+            a.ref[oN + i] = st;
+            const double c = (i > 0 && i < N - 1) ? pqp::map_distance(m, st.x, st.y) : 0.0;
+            pqp::tension_qp_station(N, i, st, c, a.w, e0 + incl - cnt, a.A_col + 4 * on, a.A_val + 4 * on, a.l + on,
+                                    a.u + on, a.Pd + on, a.Po_idx + P * on, a.Po_val + P * on, a.csc_ptr + op,
+                                    a.csc_row + oz, a.csc_val + oz);
+            for (int t = 0; t < 3; ++t) a.out_idx[3 * (oN + i) + t] = 3 * i + t;
+        }
+        e0 += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    if (lane == 0) {
+        int32_t *mb = a.meta + (size_t)pqp::kGenMeta * b;
+        const int M = pqp::tension_qp_separators(N, a.sep + 32 * (size_t)b);
+        for (int k = 0; k < pqp::kGenMeta; ++k) mb[k] = 0;
+        mb[0] = 3 * N; mb[1] = 3 * N; mb[2] = 3 * N; mb[3] = 9; mb[4] = M; mb[5] = N;
+        mb[6] = (int32_t)oN; mb[7] = (int32_t)on; mb[8] = (int32_t)on; mb[9] = (int32_t)oz; mb[10] = (int32_t)op;
     }
 }
 
@@ -1509,11 +1578,18 @@ int pqp_post_smooth_device(pqp_handle *h, int batch, const int32_t *d_knot_offse
 }
 
 namespace {
-// Carves the smoothing scratch for B paths of Km raw samples and Nm stations and `total` kept points out of one blob.
-size_t smooth_carve(char *base, int B, int Km, int Nm, int total, SmoothArgs *a) {
+// The per-station sizes of a smoothing QP in the scratch: unknowns, P partners per unknown, CSC entries.
+struct SmoothDims {
+    int n, partners, nnz;
+};
+constexpr SmoothDims kTension2Dims{4, 2, 9}, kTensionDims{3, pqp::kTensionPartners, 5};
+
+// Carves the smoothing scratch for B paths of Km raw samples and Nm stations of QP sizes d and `total` kept points out
+// of one blob.
+size_t smooth_carve(char *base, int B, int Km, int Nm, int total, const SmoothDims &d, SmoothArgs *a) {
     size_t off = 0;
     auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += (bytes + 255) & ~(size_t)255; return p; };
-    const size_t b = (size_t)B, K = (size_t)Km, N = (size_t)Nm;
+    const size_t b = (size_t)B, K = (size_t)Km, N = (size_t)Nm, n = (size_t)d.n * N;
     a->raw = (pqp_state *)take(b * K * sizeof(pqp_state));
     a->raw_off = (int32_t *)take((2 * b + 1) * sizeof(int32_t));
     a->raw_ok = (int32_t *)take(2 * b * sizeof(int32_t));
@@ -1528,13 +1604,13 @@ size_t smooth_carve(char *base, int B, int Km, int Nm, int total, SmoothArgs *a)
     a->A_val = (double *)take(b * 3 * N * 4 * sizeof(double));
     a->l = (double *)take(b * 3 * N * sizeof(double));
     a->u = (double *)take(b * 3 * N * sizeof(double));
-    a->Pd = (double *)take(b * 4 * N * sizeof(double));
-    a->q = (double *)take(b * 4 * N * sizeof(double));
-    a->Po_idx = (int32_t *)take(b * 4 * N * 2 * sizeof(int32_t));
-    a->Po_val = (double *)take(b * 4 * N * 2 * sizeof(double));
-    a->csc_ptr = (int32_t *)take(b * (4 * N + 1) * sizeof(int32_t));
-    a->csc_row = (int32_t *)take(b * 9 * N * sizeof(int32_t));
-    a->csc_val = (double *)take(b * 9 * N * sizeof(double));
+    a->Pd = (double *)take(b * n * sizeof(double));
+    a->q = (double *)take(b * n * sizeof(double));
+    a->Po_idx = (int32_t *)take(b * n * d.partners * sizeof(int32_t));
+    a->Po_val = (double *)take(b * n * d.partners * sizeof(double));
+    a->csc_ptr = (int32_t *)take(b * (n + 1) * sizeof(int32_t));
+    a->csc_row = (int32_t *)take(b * d.nnz * N * sizeof(int32_t));
+    a->csc_val = (double *)take(b * d.nnz * N * sizeof(double));
     a->sep = (int32_t *)take(b * 32 * sizeof(int32_t));
     a->out_idx = (int32_t *)take(b * N * 3 * sizeof(int32_t));
     a->frenet = (double *)take(b * N * 3 * sizeof(double));
@@ -1543,35 +1619,41 @@ size_t smooth_carve(char *base, int B, int Km, int Nm, int total, SmoothArgs *a)
     a->compact = (pqp_state *)take((size_t)total * sizeof(pqp_state));
     return off;
 }
-}  // namespace
 
-int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point_offsets, const pqp_state *d_points,
-                                double deviation_w, double curvature_w, double curvature_rate_w, int max_raw_samples,
-                                int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
-                                double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
-                                int32_t *d_status, int32_t *d_iters, void *stream) {
+// Shared memory of one path's smoothing QP of Nm stations (TENSION: 57 Nm + 13 248 doubles).
+size_t smooth_smem(bool tension, int Nm) {
+    return (tension ? pqp::gen_smem_doubles<9>(3 * Nm, 3 * Nm, 9) : pqp::gen_smem_doubles<4>(4 * Nm - 1, 3 * Nm - 1, 4)) *
+           sizeof(double);
+}
+
+// The launcher of both smoothing entries: the eight launches of the stage, the TENSION QP (with the map set and the
+// per-path index d_map_index) when `tension`, else the TENSION2 QP.
+int smooth_launch(pqp_handle *h, const char *entry, bool tension, int batch, const int32_t *d_point_offsets,
+                  const pqp_state *d_points, double deviation_w, double curvature_w, double curvature_rate_w,
+                  const int32_t *d_map_index, int max_raw_samples, int max_points, int capacity,
+                  int32_t *d_knot_offsets_out, double *d_knots_out, double *d_x_coef_out, double *d_y_coef_out,
+                  double *d_max_s_out, int32_t *d_ok, int32_t *d_status, int32_t *d_iters, void *stream) {
     auto weight_ok = [](double v) { return v >= 0 && isfinite(v); };
     if (!h || batch < 0 || capacity < 0 || max_raw_samples < 3 || max_points < 3 || !weight_ok(deviation_w) ||
         !weight_ok(curvature_w) || !weight_ok(curvature_rate_w) ||
         (batch > 0 && (!d_point_offsets || !d_points || !d_knot_offsets_out || !d_knots_out || !d_x_coef_out ||
                        !d_y_coef_out || !d_max_s_out || !d_ok || !d_status || !d_iters))) {
-        pqp_set_err("pqp_smooth_reference_device: bad argument");
+        pqp_set_err("%s: bad argument", entry);
         return PQP_ERR_ARG;
     }
     if (batch > h->max_batch || capacity > h->max_total) {
         pqp_set_err("batch / capacity exceed what the handle was created for (max_batch, max_total_points)");
         return PQP_ERR_CAPACITY;
     }
-    if (max_points > (1 << 20) ||
-        pqp::gen_smem_doubles<4>(4 * max_points - 1, 3 * max_points - 1, 4) * sizeof(double) > (size_t)h->smem_optin ||
+    if (max_points > (1 << 20) || smooth_smem(tension, max_points) > (size_t)h->smem_optin ||
         (size_t)h->max_batch * 9 * max_points > (size_t)INT32_MAX ||
         (size_t)h->max_batch * max_raw_samples > (size_t)INT32_MAX) {
-        pqp_set_err("pqp_smooth_reference_device: max_points too large for the smoothing QP of one path on one SM, or "
-                    "max_batch x max_raw_samples / max_points beyond 32-bit offsets");
+        pqp_set_err("%s: max_points too large for the smoothing QP of one path on one SM, or "
+                    "max_batch x max_raw_samples / max_points beyond 32-bit offsets", entry);
         return PQP_ERR_CAPACITY;
     }
     EnvState *e;
-    int rc = env_get(h, &e);
+    int rc = tension ? need_map(h, &e) : env_get(h, &e);
     if (rc != PQP_OK) return rc;
     PQP_CUDA(cudaSetDevice(h->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
@@ -1580,8 +1662,9 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
         return PQP_OK;
     }
     SmoothArgs a{};
+    const SmoothDims &dims = tension ? kTensionDims : kTension2Dims;
     const int Km = std::max(max_raw_samples, e->sm_raw), Nm = std::max(max_points, e->sm_points);
-    const size_t need = smooth_carve(nullptr, h->max_batch, Km, Nm, h->max_total, &a) + 2 * (size_t)h->max_batch * 4;
+    const size_t need = smooth_carve(nullptr, h->max_batch, Km, Nm, h->max_total, dims, &a) + 2 * (size_t)h->max_batch * 4;
     if (need > e->sm_cap) {
         if (e->d_sm) h->retired.push_back(e->d_sm);
         e->d_sm = nullptr;
@@ -1592,7 +1675,7 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
         e->sm_points = Nm;
     }
     if (!e->d_fit) PQP_CUDA(cudaMalloc(&e->d_fit, (size_t)h->max_total * 4 * sizeof(double)));
-    const size_t carved = smooth_carve(e->d_sm, h->max_batch, max_raw_samples, max_points, h->max_total, &a);
+    const size_t carved = smooth_carve(e->d_sm, h->max_batch, max_raw_samples, max_points, h->max_total, dims, &a);
     int32_t *n_points = (int32_t *)(e->d_sm + carved), *fit_ok = n_points + h->max_batch;
     a.w = pqp::SmoothWeights{deviation_w, curvature_w, curvature_rate_w};
     a.batch = batch; a.max_raw = max_raw_samples; a.max_points = max_points;
@@ -1603,7 +1686,8 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
     const FitArgs ra{2 * batch, a.raw_off, a.raw, a.raw_knots, a.raw_xc, a.raw_yc, a.raw_scr, a.raw_ok};
     pqp_fit_splines_kernel<<<(2 * batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(ra);
     PQP_CUDA(cudaGetLastError());
-    pqp_smooth_assemble_kernel<<<batch, 32, 0, st>>>(a);
+    if (tension) pqp_smooth_tension_assemble_kernel<<<batch, 32, 0, st>>>(a, map_table(e, d_map_index));
+    else pqp_smooth_assemble_kernel<<<batch, 32, 0, st>>>(a);
     PQP_CUDA(cudaGetLastError());
     pqp::GenView gv;
     gv.batch = batch; gv.meta = a.meta; gv.A_col = a.A_col; gv.A_val = a.A_val; gv.l = a.l; gv.u = a.u; gv.Pd = a.Pd;
@@ -1611,11 +1695,12 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
     gv.sep = a.sep; gv.out_idx = a.out_idx; gv.ref = a.ref; gv.out_states = a.smooth; gv.out_frenet = a.frenet;
     gv.status = d_status; gv.iters = d_iters;
     {
-        const size_t smem = pqp::gen_smem_doubles<4>(4 * max_points - 1, 3 * max_points - 1, 4) * sizeof(double);
+        const size_t smem = smooth_smem(tension, max_points);
         int smem_doubles = (int)(smem / sizeof(double));
         const double *q = a.q;
         void *args[] = {(void *)&h->dprm, (void *)&gv, (void *)&smem_doubles, (void *)&q};
-        PQP_CUDA(cudaLaunchKernel(pqp_gen4_kernel_fn(), dim3(batch), dim3(32), args, smem, st));
+        PQP_CUDA(cudaLaunchKernel(tension ? pqp_gen9_kernel_fn() : pqp_gen4_kernel_fn(), dim3(batch), dim3(32), args,
+                                  smem, st));
     }
     const int grid = (batch + kSmoothThreads - 1) / kSmoothThreads;
     pqp_smooth_keep_kernel<<<grid, kSmoothThreads, 0, st>>>(a);
@@ -1631,6 +1716,30 @@ int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point
     pqp_fit_splines_kernel<<<(batch + kFitPaths - 1) / kFitPaths, 2 * kFitPaths, 0, st>>>(fa);
     PQP_CUDA(cudaGetLastError());
     return PQP_OK;
+}
+}  // namespace
+
+int pqp_smooth_reference_device(pqp_handle *h, int batch, const int32_t *d_point_offsets, const pqp_state *d_points,
+                                double deviation_w, double curvature_w, double curvature_rate_w, int max_raw_samples,
+                                int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
+                                double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
+                                int32_t *d_status, int32_t *d_iters, void *stream) {
+    return smooth_launch(h, "pqp_smooth_reference_device", false, batch, d_point_offsets, d_points, deviation_w,
+                         curvature_w, curvature_rate_w, nullptr, max_raw_samples, max_points, capacity,
+                         d_knot_offsets_out, d_knots_out, d_x_coef_out, d_y_coef_out, d_max_s_out, d_ok, d_status,
+                         d_iters, stream);
+}
+
+int pqp_smooth_reference_tension_device(pqp_handle *h, int batch, const int32_t *d_point_offsets,
+                                        const pqp_state *d_points, double deviation_w, double curvature_w,
+                                        double curvature_rate_w, const int32_t *d_map_index, int max_raw_samples,
+                                        int max_points, int capacity, int32_t *d_knot_offsets_out, double *d_knots_out,
+                                        double *d_x_coef_out, double *d_y_coef_out, double *d_max_s_out, int32_t *d_ok,
+                                        int32_t *d_status, int32_t *d_iters, void *stream) {
+    return smooth_launch(h, "pqp_smooth_reference_tension_device", true, batch, d_point_offsets, d_points, deviation_w,
+                         curvature_w, curvature_rate_w, d_map_index, max_raw_samples, max_points, capacity,
+                         d_knot_offsets_out, d_knots_out, d_x_coef_out, d_y_coef_out, d_max_s_out, d_ok, d_status,
+                         d_iters, stream);
 }
 
 int pqp_update_bounds_batch(pqp_handle *h, int mode, int batch, const int32_t *n_points, const pqp_state *ref,

@@ -6,8 +6,10 @@
 // rows (<= 4 entries per row, as every row of these formulations has), orders the unknowns station
 // by station so that the reduced KKT  cP + sigma D^-2 + A' W A  is banded, and marks S-unknown
 // separators (one station's unknowns) every L stations: S = 3 for "K" and "KPC", S = 4 for the TENSION2
-// smoothing QP of pqp_smooth_reference_device, whose four chains x, y, theta, k admit no 3-unknown separator.
-// That QP also has a linear cost term q (kLinear); the formulations above have q = 0.  The device part is formulation-agnostic:
+// smoothing QP of pqp_smooth_reference_device, whose four chains x, y, theta, k admit no 3-unknown separator, and
+// S = 9 (three stations) for the TENSION smoothing QP of pqp_smooth_reference_tension_device, whose reduced KKT has
+// half-bandwidth 9 in the band order (x_i, y_i, d_i) and whose P records six partners per unknown (NP = 6).
+// The TENSION2 QP also has a linear cost term q (kLinear); the others have q = 0.  The device part is formulation-agnostic:
 // OSQP's Ruiz scaling / rho classes / ADMM recurrence / termination / adaptive rho exactly as in
 // pqp_kp_core.cuh (same unscaled-weighted form, same partitioned banded LDL'), with the stencils
 // replaced by ELL row gathers and CSC column gathers.
@@ -28,8 +30,8 @@ struct GenView {
     const double *A_val;     // [sum m][4]
     const double *l, *u;     // [sum m]
     const double *Pd;        // [sum n] diagonal of P
-    const int32_t *Po_idx;   // [sum n][2] band position of an off-diagonal partner, -1 = none
-    const double *Po_val;    // [sum n][2]
+    const int32_t *Po_idx;   // [sum n][NP] band position of an off-diagonal partner, -1 = none (NP: gen_solve_qp)
+    const double *Po_val;    // [sum n][NP]
     const int32_t *csc_ptr;  // [sum (n+1)]
     const int32_t *csc_row;  // [sum nnz]
     const double *csc_val;   // [sum nnz]
@@ -41,7 +43,7 @@ struct GenView {
     int32_t *status, *iters; // [B]
 };
 
-// Per-lane reduction record of an S-wide separator: [0, S^2) Dg / Sinv (S = 3) or its LDL' factors (S = 4), [S^2, 2S^2) Off, [2S^2, 3S^2) G,
+// Per-lane reduction record of an S-wide separator: [0, S^2) Dg / Sinv (S = 3) or its LDL' factors (S > 3), [S^2, 2S^2) Off, [2S^2, 3S^2) G,
 // [3S^2, 4S^2) A, [4S^2, 5S^2) C, [5S^2, 5S^2 + S) g.  S = 3 gives kRedStride.
 template <int S> constexpr int kGenRedStride = 5 * S * S + S;
 static_assert(kGenRedStride<3> == kRedStride, "width-3 record");
@@ -144,16 +146,16 @@ PQP_DEV void gen_local_solve(const GenCtx &cx, double *v, int lo, int hi) {
 }
 
 // band assembly (one thread per band row, deterministic) + partitioned factorisation
-template <int S>
+template <int S, int NP>
 PQP_DEV int gen_factor(Warp &w, GenCtx &cx, double cost_c) {
     constexpr int RS = kGenRedStride<S>, S2 = S * S;
     const int n = cx.n, bw = cx.bw, lane = w.lane();
     for (int j = lane; j < n; j += 32) {
         for (int dd = 0; dd <= bw; ++dd) PQP_GB(j, dd) = 0.0;
         double dg = cost_c * cx.Pd[j] + cx.sg[j];
-        for (int q = 0; q < 2; ++q) {
-            const int k = cx.Po_idx[2 * j + q];
-            if (k >= 0 && k < j) PQP_GB(j, j - k) += cost_c * cx.Po_val[2 * j + q];
+        for (int q = 0; q < NP; ++q) {
+            const int k = cx.Po_idx[NP * j + q];
+            if (k >= 0 && k < j) PQP_GB(j, j - k) += cost_c * cx.Po_val[NP * j + q];
         }
         for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
             const int r = cx.csc_row[e];
@@ -353,7 +355,9 @@ PQP_DEV bool dual_infeasible(double nrm, double qdx, double pdx, double adx_up, 
 // unscaled terms, eps = eps_dual_inf).  It runs after the SOLVED and primal-infeasibility tests, when the dual residual
 // fails, in the exact check (PQP_DUAL_INFEASIBLE) and in the x10 re-check at max_iter (PQP_DUAL_INFEASIBLE_INACCURATE).
 // dx is parked in tmp, which gen_solve leaves free until the next solve.  With q = 0, q'dx < 0 never holds.
-template <int S = 3, bool kLinear = false>
+// NP: the off-diagonal P partners recorded per unknown (Po_idx / Po_val rows): 2 for the formulations above, 6 for the
+// TENSION smoothing QP, whose x and y chains couple every unknown to three neighbours on each side.
+template <int S = 3, bool kLinear = false, int NP = 2>
 PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int prob, double *smem, size_t smem_cap,
                           const double *q = nullptr) {
     const int lane = w.lane();
@@ -367,7 +371,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
     cx.n = n; cx.m = m; cx.bw = bw; cx.M = M;
     cx.A_col = gv.A_col + 4 * (size_t)offm; cx.A_val = gv.A_val + 4 * (size_t)offm;
     cx.l = gv.l + offm; cx.u = gv.u + offm; cx.Pd = gv.Pd + offn;
-    cx.Po_idx = gv.Po_idx + 2 * (size_t)offn; cx.Po_val = gv.Po_val + 2 * (size_t)offn;
+    cx.Po_idx = gv.Po_idx + NP * (size_t)offn; cx.Po_val = gv.Po_val + NP * (size_t)offn;
     cx.csc_ptr = gv.csc_ptr + offp; cx.csc_row = gv.csc_row + offz; cx.csc_val = gv.csc_val + offz;
     cx.sep = gv.sep + 32 * (size_t)prob;
     const double *qv = kLinear ? q + offn : nullptr;
@@ -404,9 +408,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
             for (int j = lane; j < n; j += 32) {
                 const double Dj = cx.D[j];
                 double nrm = cost_c * fabs(cx.Pd[j]) * Dj * Dj;
-                for (int q = 0; q < 2; ++q) {
-                    const int k = cx.Po_idx[2 * j + q];
-                    if (k >= 0) nrm = fmax(nrm, cost_c * fabs(cx.Po_val[2 * j + q]) * Dj * cx.D[k]);
+                for (int q = 0; q < NP; ++q) {
+                    const int k = cx.Po_idx[NP * j + q];
+                    if (k >= 0) nrm = fmax(nrm, cost_c * fabs(cx.Po_val[NP * j + q]) * Dj * cx.D[k]);
                 }
                 double an = 0.0;
                 for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e)
@@ -430,9 +434,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
             for (int j = lane; j < n; j += 32) {
                 const double Dj = cx.D[j];
                 double nrm = cost_c * fabs(cx.Pd[j]) * Dj * Dj;
-                for (int q = 0; q < 2; ++q) {
-                    const int k = cx.Po_idx[2 * j + q];
-                    if (k >= 0) nrm = fmax(nrm, cost_c * fabs(cx.Po_val[2 * j + q]) * Dj * cx.D[k]);
+                for (int q = 0; q < NP; ++q) {
+                    const int k = cx.Po_idx[NP * j + q];
+                    if (k >= 0) nrm = fmax(nrm, cost_c * fabs(cx.Po_val[NP * j + q]) * Dj * cx.D[k]);
                 }
                 part += nrm;
             }
@@ -454,7 +458,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
         double rho = fmin(fmax(pm.rho, kRhoMin), kRhoMax);
         for (int r = lane; r < m; r += 32) cx.W[r] = rho_bar(cx.E[r] * cx.l[r], cx.E[r] * cx.u[r], rho) * cx.E[r] * cx.E[r];
         w.sync();
-        if (!gen_factor<S>(w, cx, cost_c)) status = PQP_NON_CVX;
+        if (!gen_factor<S, NP>(w, cx, cost_c)) status = PQP_NON_CVX;
         const double alpha = pm.alpha;
         Residuals res{};   // of the last check
         // dual-infeasibility certificate of the last check (kLinear), at eps_dual_inf and at 10 eps_dual_inf
@@ -517,9 +521,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                 double dr = 0, npx = 0, naty = 0, drs = 0, npxs = 0, natys = 0, nq = 0, nqs = 0;
                 for (int j = lane; j < n; j += 32) {
                     double px = cx.Pd[j] * cx.xr[j];
-                    for (int q = 0; q < 2; ++q) {
-                        const int k = cx.Po_idx[2 * j + q];
-                        if (k >= 0) px += cx.Po_val[2 * j + q] * cx.xr[k];
+                    for (int q = 0; q < NP; ++q) {
+                        const int k = cx.Po_idx[NP * j + q];
+                        if (k >= 0) px += cx.Po_val[NP * j + q] * cx.xr[k];
                     }
                     double aty = 0.0;
                     for (int e = cx.csc_ptr[j]; e < cx.csc_ptr[j + 1]; ++e) {
@@ -575,9 +579,9 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                         for (int j = lane; j < n; j += 32) {
                             const double dx = cx.tmp[j];
                             double p = cx.Pd[j] * dx;
-                            for (int q = 0; q < 2; ++q) {
-                                const int k = cx.Po_idx[2 * j + q];
-                                if (k >= 0) p += cx.Po_val[2 * j + q] * cx.tmp[k];
+                            for (int q = 0; q < NP; ++q) {
+                                const int k = cx.Po_idx[NP * j + q];
+                                if (k >= 0) p += cx.Po_val[NP * j + q] * cx.tmp[k];
                             }
                             dn = fmax(dn, fabs(dx)); qd += qv[j] * dx; pd = fmax(pd, fabs(p));
                         }
@@ -612,7 +616,7 @@ PQP_DEV void gen_solve_qp(Warp &w, const DevParams &pm, const GenView &gv, int p
                         }
                         rho = rho_new;
                         w.sync();
-                        if (!gen_factor<S>(w, cx, cost_c)) status = PQP_NON_CVX;
+                        if (!gen_factor<S, NP>(w, cx, cost_c)) status = PQP_NON_CVX;
                     }
                 }
             }

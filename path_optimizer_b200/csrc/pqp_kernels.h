@@ -35,4 +35,5 @@ PQP_DECLARE_VARIANT(kk_13)
 PQP_DECLARE_VARIANT(k1_generic)
 const void *pqp_gen_kernel_fn();
 const void *pqp_gen4_kernel_fn();    // the same core with 4-unknown separators and a linear cost (pqp_kgen4.cu)
+const void *pqp_gen9_kernel_fn();    // the same core with 9-unknown separators and six P partners (pqp_kgen9.cu)
 void pqp_k1_set_smem_cap(int bytes);   // device's opt-in shared memory per block (decides where the one-warp kernel keeps its scalings)

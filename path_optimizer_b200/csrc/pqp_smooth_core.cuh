@@ -1,7 +1,8 @@
-// pqp_smooth_core.cuh -- per-thread device functions of pqp_smooth_reference_device: the B-spline pre-pass of
-// ReferencePathSmoother::bSpline, the resampling of segmentRawReference and the TENSION2 smoothing QP of
-// TensionSmoother2::osqpSmooth, assembled in the band order of the generic core (pqp_gen_core.cuh, 4-unknown
-// separators).  Like pqp_corridor_core.cuh, every function is a straight per-thread restatement, so the test-only host
+// pqp_smooth_core.cuh -- per-thread device functions of pqp_smooth_reference_device and
+// pqp_smooth_reference_tension_device: the B-spline pre-pass of ReferencePathSmoother::bSpline, the resampling of
+// segmentRawReference, the TENSION2 smoothing QP of TensionSmoother2::osqpSmooth and the TENSION smoothing QP of
+// TensionSmoother::osqpSmooth, assembled in the band order of the generic core (pqp_gen_core.cuh, 4-unknown
+// separators for TENSION2, 9-unknown separators for TENSION).  Like pqp_corridor_core.cuh, every function is a straight per-thread restatement, so the test-only host
 // build (-DPQP_HOST_EMU, tests/emu/) calls them in a loop where the kernel spreads them over a warp.
 //
 // Reference behaviour being replaced (file:line in the reference tree):
@@ -10,6 +11,8 @@
 //   ReferencePathSmoother::segmentRawReference         :50-88
 //   TensionSmoother2::osqpSmooth / setHessianMatrix / setConstraintMatrix / setGradient
 //                                                      src/reference_path_smoother/tension_smoother_2.cpp:163-301
+//   TensionSmoother::osqpSmooth / setHessianMatrix / setConstraintMatrix
+//                                                      src/reference_path_smoother/tension_smoother.cpp:186-314
 //   TensionSmoother::smooth tail                       src/reference_path_smoother/tension_smoother.cpp:84-96
 //   distance                                           src/tools/tools.cpp:46-48
 //
@@ -35,7 +38,8 @@ enum SmoothRefusal {
     SM_SHORT = 7,        // fewer than 3 resampled stations (the smoothed spline's tk::spline::set_points)
     SM_QP = 8,           // the smoothing QP did not end SOLVED
     SM_S_ORDER = 9,      // the smoothed s is not strictly increasing or not finite (tk::spline::set_points)
-    SM_CAPACITY = 10     // the running knot total would pass the capacity (decided by the reservation)
+    SM_CAPACITY = 10,    // the running knot total would pass the capacity (decided by the reservation)
+    SM_MAP = 11          // TENSION: the path's map index lies outside the map set
 };
 
 constexpr int kSmoothMaxDegree = 5;
@@ -191,6 +195,119 @@ PQP_HD int smooth_qp_separators(int N, int32_t *sep) {
     if (L < 2) L = 2;
     int M = 0;
     for (int e = 0; e < N - 1 && M < 32; e += L) sep[M++] = 4 * e;
+    return M;
+}
+
+// The TENSION QP (TensionSmoother::setHessianMatrix / setConstraintMatrix, tension_smoother.cpp:239-314; q = 0) in the
+// band order of the generic core: station i's unknowns (x_i, y_i, d_i) at 3i .. 3i + 2, n = 3N; rows in the
+// reference's order -- x_i - cos(theta_i) d_i = x_ref_i (row i), y_i - sin(theta_i) d_i = y_ref_i (N + i), d_i (2N + i),
+// m = 3N, theta_i = heading_i + pi/2 unwrapped.  The x and y chains of P couple each unknown to three neighbours on each
+// side, so the reduced KKT has half-bandwidth 9 and a separator is three stations (9 unknowns).  Weights: w = (deviation,
+// curvature, curvature rate) = FLAGS_cartesian_deviation_weight, _curvature_weight, _curvature_rate_weight.  Exact zeros
+// of P and A are dropped, as Eigen's sparseView drops them.
+constexpr int kTensionPartners = 6;
+constexpr double kTensionHalfPi = 1.57079632679489661923;   // M_PI_2
+constexpr double kTensionMaxClearance = 2.0;                  // default_clearance (:300)
+
+// (1, -2, 1) and (-1, 3, -3, 1), the dds and ddds vectors of setHessianMatrix
+PQP_HD double tension_dds(int k) { return k == 1 ? -2.0 : 1.0; }
+PQP_HD double tension_ddds(int k) { return k == 0 ? -1.0 : k == 1 ? 3.0 : k == 2 ? -3.0 : 1.0; }
+
+// Entry (a, b), |a - b| <= 3, of the x (or y) chain of setHessianMatrix (:245-257): the dds block (v_a v_b) w_curv at
+// i = 0 .. N - 3 and the ddds block (u_a u_b) w_rate at i = 0 .. N - 4, added into a zero matrix in the reference's
+// order (block i's dds, then its ddds), each block entry rounded once.
+PQP_HD double tension_chain_hess(int N, int a, int b, const SmoothWeights &w) {
+    const int lo = a < b ? a : b, hi = a < b ? b : a;
+    double h = 0.0;
+    for (int i = hi - 3 > 0 ? hi - 3 : 0; i <= lo && i <= N - 3; ++i) {
+        if (hi - i <= 2) h = add(h, mul(mul(tension_dds(a - i), tension_dds(b - i)), w.curv));
+        if (i <= N - 4) h = add(h, mul(mul(tension_ddds(a - i), tension_ddds(b - i)), w.rate));
+    }
+    return h;
+}
+
+// The d_i column's cos / sin entries of rows x_i and y_i: -cos(theta_i), -sin(theta_i) (:283-285).
+PQP_HD void tension_normal(const pqp_state &st, double *nc, double *ns) {
+    const double theta = add(st.z, kTensionHalfPi);
+    *nc = -cos(theta);
+    *ns = -sin(theta);
+}
+
+// Station i's CSC entries: x_i and y_i one each, d_i its kept cos / sin entries and its own row.
+PQP_HD int tension_qp_csc_count(const pqp_state &st) {
+    double nc, ns;
+    tension_normal(st, &nc, &ns);
+    return 3 + (nc != 0.0) + (ns != 0.0);
+}
+
+// Station i's entries: its rows x_i, y_i, d_i, its P entries and its CSC columns.  st: the resampled station (x, y,
+// heading z); clearance: Map::getObstacleDistance at (st.x, st.y), read for 0 < i < N - 1 only; e: the CSC entries of
+// stations 0 .. i - 1 (tension_qp_csc_count summed).  A_col / A_val / l / u point at the path's rows, Pd / Po_idx /
+// Po_val [kTensionPartners] at its n-arrays (partners in ascending band position, unused slots -1), ptr / row / val at
+// its CSC arrays; the last station also closes ptr[3N].
+PQP_HD void tension_qp_station(int N, int i, const pqp_state &st, double clearance, const SmoothWeights &w, int e,
+                               int32_t *A_col, double *A_val, double *l, double *u, double *Pd, int32_t *Po_idx,
+                               double *Po_val, int32_t *ptr, int32_t *row, double *val) {
+    double nc, ns;
+    tension_normal(st, &nc, &ns);
+    const int g = 3 * i;
+    auto put = [&](int r, int c0, int c1, double v1, double lo, double up) {
+        A_col[4 * r] = c0; A_val[4 * r] = 1.0;
+        const bool keep = c1 >= 0 && v1 != 0.0;
+        A_col[4 * r + 1] = keep ? c1 : -1; A_val[4 * r + 1] = keep ? v1 : 0.0;
+        A_col[4 * r + 2] = A_col[4 * r + 3] = -1;
+        A_val[4 * r + 2] = A_val[4 * r + 3] = 0.0;
+        l[r] = lo; u[r] = up;
+    };
+    put(i, g, g + 2, nc, st.x, st.x);
+    put(N + i, g + 1, g + 2, ns, st.y, st.y);
+    // d bounds (:296-313): d_0 = 0, |d_{N-1}| <= 0.5, otherwise |d_i| <= std::min(clearance, 2)
+    double dl = 0.0, du = 0.0;
+    if (i == N - 1) { dl = -0.5; du = 0.5; }
+    else if (i > 0) {
+        const double c = kTensionMaxClearance < clearance ? kTensionMaxClearance : clearance;
+        dl = -c; du = c;
+    }
+    put(2 * N + i, g + 2, -1, 0.0, dl, du);
+    // P: the x and y chains (x_k at 3k, y_k at 3k + 1), then d_i's diagonal w_dev (:258-261)
+    for (int t = 0; t < 2; ++t) {
+        const int j = g + t;
+        Pd[j] = tension_chain_hess(N, i, i, w);
+        int q = 0;
+        for (int k = i - 3; k <= i + 3; ++k) {
+            if (k < 0 || k >= N || k == i) continue;
+            const double h = tension_chain_hess(N, i, k, w);
+            if (h != 0.0) { Po_idx[kTensionPartners * j + q] = 3 * k + t; Po_val[kTensionPartners * j + q] = h; ++q; }
+        }
+        for (; q < kTensionPartners; ++q) { Po_idx[kTensionPartners * j + q] = -1; Po_val[kTensionPartners * j + q] = 0.0; }
+    }
+    Pd[g + 2] = w.dev;
+    for (int q = 0; q < kTensionPartners; ++q) {
+        Po_idx[kTensionPartners * (g + 2) + q] = -1;
+        Po_val[kTensionPartners * (g + 2) + q] = 0.0;
+    }
+    // CSC, rows ascending: x_i (row i), y_i (row N + i), d_i (rows i, N + i, 2N + i)
+    ptr[g] = e;
+    row[e] = i; val[e++] = 1.0;
+    ptr[g + 1] = e;
+    row[e] = N + i; val[e++] = 1.0;
+    ptr[g + 2] = e;
+    if (nc != 0.0) { row[e] = i; val[e++] = nc; }
+    if (ns != 0.0) { row[e] = N + i; val[e++] = ns; }
+    row[e] = 2 * N + i; val[e++] = 1.0;
+    if (i == N - 1) ptr[3 * N] = e;
+}
+
+// The generic core's separators for the TENSION QP: stations e, e + 1, e + 2 (band positions 3e .. 3e + 8) for e = 0,
+// L, 2L, ... with e + 2 < N - 1, at most 32, L = max(6, (N - 4) / 31 + 1).  L >= 6 leaves at least three stations (9
+// unknowns, the half-bandwidth) between two separators, so no entry of the reduced KKT couples two separators; the first
+// always starts at 0.  Returns M.
+PQP_HD int tension_qp_separators(int N, int32_t *sep) {
+    int L = (N - 4) / 31 + 1;
+    if (L < 6) L = 6;
+    int M = 0;
+    sep[M++] = 0;
+    for (int e = L; e + 3 <= N - 1 && M < 32; e += L) sep[M++] = 3 * e;
     return M;
 }
 

@@ -22,6 +22,9 @@ from .solver import BatchPathSolver, PqpError
 
 BOUNDS_IMPROVED, BOUNDS_SIMPLE = 0, 1
 OUTPUT_RAW, OUTPUT_DENSIFY = 0, 1
+# smooth_device: the deviation, curvature and curvature-rate weights of each smoothing method under the reference's
+# default flags (FLAGS_tension_2_* and FLAGS_cartesian_*, planning_flags.cpp:72-82)
+SMOOTH_WEIGHTS = {"TENSION2": (0.005, 1.0, 10.0), "TENSION": (0.0, 1.0, 50.0)}
 
 
 def update_limits(params, ref, from_spline=False):
@@ -388,19 +391,27 @@ class PathPlanner(BatchPathSolver):
         return dict(knot_offsets=ko, knots=kn, x_coef=xc, y_coef=yc, max_s=ms, ok=ok, status=status, iters=iters,
                     layers=layers)
 
-    def smooth_device(self, points, point_offsets, max_raw_samples, max_points, capacity=None, weights=(0.005, 1, 10),
-                      out=None):
-        """ReferencePathSmoother's B-spline pre-pass and TENSION2 smoothing QP for every raw polyline of a batch on the
-        device (pqp_smooth_reference_device): raw polylines in, smoothed lines out in the layout post_smooth_device
-        reads as `splines`.  points float64 [P, 7] (x and y read), point_offsets int32 [B + 1], torch CUDA tensors; on
-        torch.cuda.current_stream().  max_raw_samples: B-spline samples a path may have at most; max_points: stations
-        a path may have at most; capacity: knot rows of the output (default the planner's max_total_points); weights:
-        FLAGS_tension_2_deviation_weight, _curvature_weight, _curvature_rate_weight.  Returns dict(knot_offsets int32
-        [B + 1], knots [capacity], x_coef / y_coef [capacity, 4], max_s [B], ok, status, iters int32 [B]).  A refused
-        path gets ok = 0, 0 knots and NaN max_s.  No host synchronisation; after one call with the largest caps it can
-        be captured in a CUDA graph.  `out` may carry the output tensors, e.g. those of an earlier call."""
+    def smooth_device(self, points, point_offsets, max_raw_samples, max_points, capacity=None, weights=None, out=None,
+                      method="TENSION2", map_index=None):
+        """ReferencePathSmoother's B-spline pre-pass and smoothing QP for every raw polyline of a batch on the device:
+        raw polylines in, smoothed lines out in the layout post_smooth_device reads as `splines`.  points float64 [P, 7]
+        (x and y read), point_offsets int32 [B + 1], torch CUDA tensors; on torch.cuda.current_stream().
+        max_raw_samples: B-spline samples a path may have at most; max_points: stations a path may have at most;
+        capacity: knot rows of the output (default the planner's max_total_points).  method: FLAGS_smoothing_method,
+        "TENSION2" (pqp_smooth_reference_device) or "TENSION" (pqp_smooth_reference_tension_device, whose QP bounds each
+        station's offset by its clearance in the map set of set_map / set_maps).  weights: the method's deviation,
+        curvature and curvature-rate weights -- FLAGS_tension_2_* (default (0.005, 1, 10)) or FLAGS_cartesian_*
+        (default (0, 1, 50)).  map_index: int32 [B] CUDA tensor, the map of every path (TENSION only; None: map 0).
+        Returns dict(knot_offsets int32 [B + 1], knots [capacity], x_coef / y_coef [capacity, 4], max_s [B], ok, status,
+        iters int32 [B]).  A refused path gets ok = 0, 0 knots and NaN max_s.  No host synchronisation; after one call
+        with the largest caps it can be captured in a CUDA graph.  `out` may carry the output tensors, e.g. those of an
+        earlier call."""
         import torch
         from . import device as D
+        if method not in SMOOTH_WEIGHTS:
+            raise ValueError(f"smoothing method {method!r}: expected one of {sorted(SMOOTH_WEIGHTS)}")
+        if map_index is not None and method != "TENSION":
+            raise ValueError(f"map_index is read by the TENSION smoother only, not by {method}")
         dev = self._cuda_device()
         B = int(point_offsets.shape[0]) - 1
         P = int(points.shape[0])
@@ -413,17 +424,22 @@ class PathPlanner(BatchPathSolver):
         ko, kn = buf("knot_offsets", (B + 1,), i32), buf("knots", (cap,), f64)
         xc, yc, ms = buf("x_coef", (cap, 4), f64), buf("y_coef", (cap, 4), f64), buf("max_s", (B,), f64)
         ok, status, iters = buf("ok", (B,), i32), buf("status", (B,), i32), buf("iters", (B,), i32)
-        w_dev, w_curv, w_rate = (float(v) for v in weights)
-        rc = self._L.pqp_smooth_reference_device(
-            self._h, B, D.check(point_offsets, "point_offsets", i32, (B + 1,), dev),
-            D.check(points, "points", f64, (P, D.STATE_COLS), dev), w_dev, w_curv, w_rate, int(max_raw_samples),
-            int(max_points), cap, D.check(ko, "knot_offsets", i32, (B + 1,), dev), D.check(kn, "knots", f64, (cap,), dev),
-            D.check(xc, "x_coef", f64, (cap, 4), dev), D.check(yc, "y_coef", f64, (cap, 4), dev),
-            D.check(ms, "max_s", f64, (B,), dev), D.check(ok, "ok", i32, (B,), dev),
-            D.check(status, "status", i32, (B,), dev), D.check(iters, "iters", i32, (B,), dev),
-            torch.cuda.current_stream(dev).cuda_stream)
+        w_dev, w_curv, w_rate = (float(v) for v in (SMOOTH_WEIGHTS[method] if weights is None else weights))
+        head = (self._h, B, D.check(point_offsets, "point_offsets", i32, (B + 1,), dev),
+                D.check(points, "points", f64, (P, D.STATE_COLS), dev), w_dev, w_curv, w_rate)
+        if method == "TENSION":
+            entry = "pqp_smooth_reference_tension_device"
+            head += (None if map_index is None else D.check(map_index, "map_index", i32, (B,), dev),)
+        else:
+            entry = "pqp_smooth_reference_device"
+        rc = getattr(self._L, entry)(
+            *head, int(max_raw_samples), int(max_points), cap, D.check(ko, "knot_offsets", i32, (B + 1,), dev),
+            D.check(kn, "knots", f64, (cap,), dev), D.check(xc, "x_coef", f64, (cap, 4), dev),
+            D.check(yc, "y_coef", f64, (cap, 4), dev), D.check(ms, "max_s", f64, (B,), dev),
+            D.check(ok, "ok", i32, (B,), dev), D.check(status, "status", i32, (B,), dev),
+            D.check(iters, "iters", i32, (B,), dev), torch.cuda.current_stream(dev).cuda_stream)
         if rc != OK:
-            raise PqpError(f"pqp_smooth_reference_device failed (rc={rc}): {_lib.last_error()}")
+            raise PqpError(f"{entry} failed (rc={rc}): {_lib.last_error()}")
         return dict(knot_offsets=ko, knots=kn, x_coef=xc, y_coef=yc, max_s=ms, ok=ok, status=status, iters=iters)
 
     def plan_device(self, n_points, offsets, ref, x0, end_heading, max_n_points=0, formulation="KP",
